@@ -9,6 +9,10 @@
 //              lower index without risk of deadlock, whatever the residency.
 //   compact  : three-kernel stream compaction (tile counts, scan of the tile
 //              counts, in-tile scan + emit); ranks are exact and ordered.
+//   subsample_distance : warp-per-cell dataflow over the cells of a level
+//              (lod_subsample_warp.cuh), wavefront order for large levels.
+//   block_stage : one RAHT stage with the thread-per-block body; the CUDA
+//              descent is otherwise WaveDescent's (raht_wave.cuh).
 //
 // Workspace comes from a per-context arena (one cudaMalloc in steady state).
 #pragma once
@@ -328,9 +332,6 @@ struct DeviceExec {
   Profiler* prof = nullptr;
   int curPhase = 0;
   const std::atomic<int>* activeCalls = nullptr;  // calls in flight (all lanes)
-  // zero-run regions of the stages of the running call (warp block kernel)
-  TzRegion* dRegions = nullptr;
-  int numRegions = 0;
 
   void phase(int p) { curPhase = p; }
 
@@ -452,14 +453,6 @@ struct DeviceExec {
   {
     if (nCells <= 0)
       return;
-    static const bool threadMode = [] {
-      const char* e = getenv("PCCB200_BLOCK_KERNEL");
-      return e && !strcmp(e, "thread");
-    }();
-    if (threadMode) {
-      ordered(nCells, fn);
-      return;
-    }
     SubsampleCellsArgs a;
     a.v = fn.v;
     a.input = fn.input;
@@ -475,10 +468,8 @@ struct DeviceExec {
     Scope sc(*this);
     const int64_t threads = int64_t(nCells) * 19;
     k_cell_neighbours<<<unsigned((threads + 255) / 256), 256, 0, stream>>>(a);
-    // wavefront order for the large levels (see k_cell_levels); A/B knob
-    // PCCB200_SUBSAMPLE_WAVE=0: Morton order everywhere
-    const char* ew = getenv("PCCB200_SUBSAMPLE_WAVE");
-    if (nCells >= 4096 && !(ew && atoi(ew) == 0))
+    // wavefront order for the large levels (see k_cell_levels)
+    if (nCells >= 4096)
       a.order = cell_wave_order(a.nb, nCells);
     PCC_CUDA_CHECK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), stream));
     int64_t blocks = (int64_t(nCells) + 7) / 8;
@@ -490,22 +481,7 @@ struct DeviceExec {
       cap = 8;
     if (blocks > cap)
       blocks = cap;
-    // A/B knob (default off): chunks of cells per CTA with the records in shared
-    // memory -- measured an order of magnitude SLOWER per 1M-point slice: the
-    // barrier per chunk and 16 warps per 256 cells cost far more parallelism than the shorter hop returns
-    const char* ech = getenv("PCCB200_SUBSAMPLE_CHUNK");
-    if (ech && atoi(ech) != 0) {
-      int64_t chunks = (int64_t(nCells) + kCellChunk - 1) / kCellChunk;
-      int64_t ccap = int64_t(numSMs) * 4;  // 4 CTAs of 512 threads per SM
-      if (inFlight > 1)
-        ccap /= 2 * inFlight;
-      if (ccap < 4)
-        ccap = 4;
-      k_subsample_cells_chunked<<<unsigned(chunks > ccap ? ccap : chunks), kCellChunkThreads, 0,
-                                  stream>>>(a, ticket);
-    } else {
-      k_subsample_cells<<<unsigned(blocks), 256, 0, stream>>>(a, ticket);
-    }
+    k_subsample_cells<<<unsigned(blocks), 256, 0, stream>>>(a, ticket);
     g_launchCount += 2;
     PCC_CUDA_CHECK(cudaGetLastError());
   }
@@ -548,101 +524,22 @@ struct DeviceExec {
     return blocks > cap ? cap : blocks;
   }
 
-  // One top-down stage.  Default: PrepFn (single-child blocks, qp descent) ->
-  // worklist of the transforming blocks -> warp-cooperative dataflow kernel.
-  // PCCB200_BLOCK_KERNEL=thread selects the thread-per-block body (BlockFn)
-  // instead, for A/B comparison.
+  // One top-down stage with the thread-per-block body (BlockFn): the stage
+  // where WaveDescent does not run, i.e. the encoder with AC-coefficient qp
+  // offsets.  Those make the RDOQ decision matter even for coefficients that
+  // quantise to zero, so that case keeps the exact zero-run counter protocol
+  // of this body, handed from stage to stage through tzNext.
   template<class Fn>
   void block_stage(const Fn& fn, int64_t nBlocks, int* tzNext)
   {
-    static const bool threadMode = [] {
-      const char* e = getenv("PCCB200_BLOCK_KERNEL");
-      return e && !strcmp(e, "thread");
-    }();
-    const bool root = fn.P.n == 0;
-    // AC-coefficient qp offsets make the RDOQ decision matter even for
-    // coefficients that quantise to zero; that (rare) case keeps the exact
-    // counter protocol of the thread-per-block body
-    const bool exactCounter = fn.cfg.isEncoder && !fn.cfg.haar && fn.cfg.numAcLayers > 0;
-    if (threadMode || exactCounter) {
-      if (root) {
-        foreach(1, fn);
-      } else {
-        foreach(nBlocks, PrepFn{fn.cfg, fn.S, fn.P, fn.predInLvl, fn.tz});
-        ordered(nBlocks, SkipSinglesFn<Fn>{fn});
-      }
-      if (tzNext)
-        foreach(1, TzCarryFn{fn.tz, nullptr, int(nBlocks), tzNext});
-      return;
-    }
-    WarpBlockArgs a = {};
-    a.cfg = fn.cfg;
-    a.numSets = 1;
-    AttrSet& st = a.set[0];
-    st.A = fn.cfg.A;
-    st.base = 0;
-    st.maxQp = fn.cfg.maxQp;
-    st.fixedPointQpOffset = fn.cfg.fixedPointQpOffset;
-    st.numAcLayers = fn.cfg.numAcLayers;
-    st.qpLayer = fn.qpLayer;
-    st.acLayer = fn.acLayer;
-    st.qt = fn.qt;
-    st.coef = fn.coef;
-    st.coefStride = fn.coefStride;
-    a.S = fn.S;
-    a.P = fn.P;
-    a.coefBase = fn.coefBase;
-    a.predInLvl = fn.predInLvl;
-    raht_ab(1, 1, a.ab11a, a.ab11b);
-    int* dCount = alloc<int>(1);
-    if (root) {
-      int one = 1;
-      upload(dCount, &one, sizeof(int));
-      a.worklist = nullptr;
+    if (fn.P.n == 0) {
+      foreach(1, fn);
     } else {
-      foreach(nBlocks, PrepFn{fn.cfg, fn.S, fn.P, fn.predInLvl, nullptr});
-      int32_t* list = alloc<int32_t>(size_t(nBlocks));
-      compact(nBlocks, MultiChildPred{fn.P.first}, WorklistEmit{list}, dCount);
-      a.worklist = list;
+      foreach(nBlocks, PrepFn{fn.cfg, fn.S, fn.P, fn.predInLvl, fn.tz});
+      ordered(nBlocks, SkipSinglesFn<Fn>{fn});
     }
-    a.count = dCount;
-    if (root || !dRegions) {
-      dRegions = alloc<TzRegion>(32);
-      numRegions = 0;
-    }
-    TzRegion hr;
-    hr.state = nullptr;
-    if (fn.tz) {  // (the encoder with RDOQ: one state word per block, zero = nothing published)
-      hr.state = alloc<unsigned long long>(size_t(nBlocks) + 1);
-      zero(hr.state, (size_t(nBlocks) + 1) * sizeof(unsigned long long));
-    }
-    hr.count = dCount;
-    a.stageIdx = numRegions;
-    upload(dRegions + numRegions, &hr, sizeof(TzRegion));
-    numRegions++;
-    st.regions = dRegions;
-    st.state = hr.state;
-    static const int pollNs = [] {
-      const char* e = getenv("PCCB200_POLL_NS");
-      return e ? atoi(e) : 32;
-    }();
-    a.pollNs = pollNs;
-    a.geom = nullptr;
-    if (!root && fn.predInLvl) {
-      a.geom = alloc<int32_t>(size_t(nBlocks) * kGeomStride);
-      Scope sc(*this);
-      k_block_geom<<<unsigned((nBlocks * 32 + 255) / 256), 256, 0, stream>>>(a);
-      g_launchCount++;
-    }
-    PCC_CUDA_CHECK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), stream));
-    const int64_t blocks = block_grid(nBlocks);
-    {
-      Scope sc(*this);
-      k_block_warp<<<unsigned(blocks), kWarpBlockThreads, 0, stream>>>(a, ticket);
-    }
-    g_launchCount++;
-    PCC_CUDA_CHECK(cudaGetLastError());
-    (void)tzNext;  // the run-length queries walk across stages themselves
+    if (tzNext)
+      foreach(1, TzCarryFn{fn.tz, nullptr, int(nBlocks), tzNext});
   }
 };
 

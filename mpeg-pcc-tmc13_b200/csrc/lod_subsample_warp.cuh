@@ -214,115 +214,4 @@ k_cell_levels(const int32_t* __restrict__ nb, const int nCells, int* lv, int64_t
   }
 }
 
-// EXPERIMENT (PCCB200_SUBSAMPLE_CHUNK=1, off by default, measured much slower than
-// k_subsample_cells: see exec_cuda.cuh).
-// The same dataflow with chunks of cells per CTA.  Consecutive cells in Morton
-// order are mostly each other's neighbours, and -- unlike the RAHT blocks --
-// a cell has next to no arithmetic of its own: the hop from a cell to the next
-// IS the L2 round trip of the neighbour's record.  So a CTA takes kCellChunk
-// consecutive cells at a time (claimed through the global ticket, in ascending
-// order), deals them to its warps round robin, and keeps the records of the
-// chunk in shared memory as well as in global memory: a neighbour inside the
-// chunk is polled in shared memory.  A barrier separates the chunks of a CTA,
-// so a slot belongs to one cell for the whole chunk.  Deadlock freedom as
-// before: chunks are claimed in ascending order by running CTAs, a warp works
-// through its cells of a chunk in ascending order, a cell waits for lower
-// cells only.
-constexpr int kCellChunk = 256;
-constexpr int kCellChunkThreads = 512;
-
-__global__ void __launch_bounds__(kCellChunkThreads)
-k_subsample_cells_chunked(const SubsampleCellsArgs a, unsigned long long* ticket)
-{
-  __shared__ int sRec[kCellChunk][4];  // x, y, z, state (kCellRec*)
-  __shared__ unsigned long long sBase;
-  const int lane = threadIdx.x & 31;
-  const int warp = threadIdx.x >> 5;
-  const int numWarps = blockDim.x >> 5;
-  const int64_t radius2 = int64_t(3) << (a.shiftBits0 << 1);
-  for (;;) {
-    if (threadIdx.x == 0)
-      sBase = atomicAdd(ticket, (unsigned long long)kCellChunk);
-    for (int i = threadIdx.x; i < kCellChunk; i += blockDim.x)
-      sRec[i][3] = kCellRecUndecided;
-    __syncthreads();
-    const unsigned long long base64 = sBase;
-    if (base64 >= (unsigned long long)a.nCells)
-      return;
-    const int base = int(base64);
-    const int end = base + kCellChunk < a.nCells ? base + kCellChunk : a.nCells;
-    for (int c = base + warp; c < end; c += numWarps) {
-      const int q = lane < 19 ? a.nb[size_t(c) * 19 + lane] : -1;
-      const int i0 = a.cellFirst[c], i1 = a.cellFirst[c + 1];
-      int32_t pa[3] = {0, 0, 0}, pb[3] = {0, 0, 0};
-      {
-        const uint32_t ia = a.input[i0];
-        const uint32_t ib = i0 + 1 < i1 ? a.input[i0 + 1] : ia;
-        const int32_t* p = &a.v.pos[size_t(ia) * 3];
-        const int32_t* r = &a.v.pos[size_t(ib) * 3];
-        pa[0] = p[0], pa[1] = p[1], pa[2] = p[2];
-        pb[0] = r[0], pb[1] = r[1], pb[2] = r[2];
-      }
-      bool have = false;
-      int32_t np[3] = {0, 0, 0};
-      if (q >= base) {  // a cell of this chunk: its record is (or will be) in shared memory
-        volatile int* r = sRec[q - base];
-        while (r[3] == kCellRecUndecided)
-          __nanosleep(20);
-        __threadfence_block();
-        if (r[3] == kCellRecPoint) {
-          np[0] = r[0], np[1] = r[1], np[2] = r[2];
-          have = true;
-        }
-      } else if (q >= 0) {
-        int4 r = ld_cell_rec(&a.decPos[q]);
-        while (r.w == kCellRecUndecided) {
-          __nanosleep(32);
-          r = ld_cell_rec(&a.decPos[q]);
-        }
-        if (r.w == kCellRecPoint) {
-          np[0] = r.x, np[1] = r.y, np[2] = r.z;
-          have = true;
-        }
-      }
-      int chosen = kCellNone;
-      for (int i = i0; i < i1; i++) {
-        int32_t pp[3];
-        if (i == i0) {
-          pp[0] = pa[0], pp[1] = pa[1], pp[2] = pa[2];
-        } else if (i == i0 + 1) {
-          pp[0] = pb[0], pp[1] = pb[1], pp[2] = pb[2];
-        } else {
-          const int32_t* p = &a.v.pos[size_t(a.input[i]) * 3];
-          pp[0] = p[0], pp[1] = p[1], pp[2] = p[2];
-        }
-        const bool hit = have && norm2_3(np, pp) <= radius2;
-        const bool found = __ballot_sync(0xffffffffu, hit) != 0;
-        if (!found) {
-          chosen = i;
-          if (lane == 0) {
-            volatile int* r = sRec[c - base];
-            r[0] = pp[0], r[1] = pp[1], r[2] = pp[2];
-            __threadfence_block();
-            r[3] = kCellRecPoint;
-            st_cell_rec(&a.decPos[c], pp[0], pp[1], pp[2], kCellRecPoint);
-            a.keep[i] = 1;
-          }
-          for (int r = i + 1 + lane; r < i1; r += 32)
-            a.keep[r] = 0;
-          break;
-        }
-        if (lane == 0)
-          a.keep[i] = 0;
-      }
-      if (chosen == kCellNone && lane == 0) {
-        volatile int* r = sRec[c - base];
-        r[3] = kCellRecNone;
-        st_cell_rec(&a.decPos[c], 0, 0, 0, kCellRecNone);
-      }
-    }
-    __syncthreads();  // the chunk is done: its slots and sBase may be reused
-  }
-}
-
 }  // namespace pccb200

@@ -185,20 +185,6 @@ k_radix_scatter(const int64_t* __restrict__ keysIn, const int32_t* __restrict__ 
   }
 }
 
-// out[i*A + k] = in[order[i]*A + k]
-template<class T>
-__global__ void __launch_bounds__(256)
-k_gather_rows(const T* __restrict__ in, const int32_t* __restrict__ order, int64_t n, int A,
-              T* __restrict__ out)
-{
-  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < n;
-       i += int64_t(gridDim.x) * blockDim.x) {
-    int64_t src = order[i];
-    for (int k = 0; k < A; k++)
-      out[i * A + k] = in[src * A + k];
-  }
-}
-
 // out[i*outStride + outOff + k] = in[order[i]*A + k]  (one attribute of several
 // into the interleaved rows of a multi-attribute pass)
 __global__ void __launch_bounds__(256)
@@ -224,22 +210,6 @@ k_scatter_rows_clip_strided(const int32_t* __restrict__ in, int inStride, int in
     int64_t dst = order[i];
     for (int k = 0; k < A; k++) {
       int32_t v = in[i * inStride + inOff + k];
-      v = v < 0 ? 0 : (v > clipMax ? clipMax : v);
-      out[dst * A + k] = v;
-    }
-  }
-}
-
-// out[order[i]*A + k] = clip(in[i*A + k], 0, clipMax)
-__global__ void __launch_bounds__(256)
-k_scatter_rows_clip(const int32_t* __restrict__ in, const int32_t* __restrict__ order,
-                    int64_t n, int A, int32_t clipMax, int32_t* __restrict__ out)
-{
-  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < n;
-       i += int64_t(gridDim.x) * blockDim.x) {
-    int64_t dst = order[i];
-    for (int k = 0; k < A; k++) {
-      int32_t v = in[i * A + k];
       v = v < 0 ? 0 : (v > clipMax ? clipMax : v);
       out[dst * A + k] = v;
     }

@@ -4,6 +4,12 @@
 // the kernels on the context's stream, copy results back, synchronise.  No
 // CPU implementation exists behind this ABI: without a usable sm_90 device
 // every compute entry point returns PCCB200_ERR_NO_DEVICE.
+//
+// The attribute-RAHT entries (single attribute, slices, several attributes,
+// batches; host or device pointers) describe their work as coding units
+// (RahtUnit) and share one pipeline: code_raht chooses fused or per-attribute
+// passes and deals the units to lanes, code_units codes a gang of them on one
+// lane.
 #include <cuda_runtime.h>
 
 #include <stdlib.h>
@@ -319,128 +325,6 @@ raht_common(bool forward, const pccb200_raht_params* params, const pccb200_qpset
   });
 }
 
-// one slice: sort, gather, transform, clip + scatter back.  All array
-// pointers are device pointers addressing the slice's first point; coefficient
-// component k sits at dCoef + k * coefStride.
-int
-attr_raht_slice(DeviceExec& ex, bool forward, const pccb200_raht_params* params,
-                const pccb200_qpset* qpset, const int32_t* dQpoIn, const int32_t* dXyz,
-                const int32_t* dAttrsIn, int32_t* dAttrsOut, int A, int bitdepth, int n,
-                int32_t* dCoef, int64_t coefStride)
-{
-  int64_t* dKeys = ex.alloc<int64_t>(size_t(n));
-  int32_t* dOrder = ex.alloc<int32_t>(size_t(n));
-  int32_t* dAttrs = ex.alloc<int32_t>(size_t(n) * A);
-  int32_t* dQpo = dQpoIn ? ex.alloc<int32_t>(size_t(n) * 2) : nullptr;
-  const int32_t clipMax = (1 << bitdepth) - 1;
-  device_morton_sort(ex, dXyz, n, dKeys, dOrder);
-  const unsigned g = grid_for(n, ex.numSMs);
-  ex.phase(kPhaseGather);
-  if (forward) {
-    DeviceExec::Scope sc(ex);
-    k_gather_rows<int32_t><<<g, 256, 0, ex.stream>>>(dAttrsIn, dOrder, n, A, dAttrs);
-    g_launchCount++;
-  }
-  if (dQpoIn) {
-    DeviceExec::Scope sc(ex);
-    k_gather_rows<int32_t><<<g, 256, 0, ex.stream>>>(dQpoIn, dOrder, n, 2, dQpo);
-    g_launchCount++;
-  }
-  int rc = raht_run(ex, *params, *qpset, forward, dKeys, dAttrs, dQpo, dCoef, coefStride, A, n);
-  if (rc != PCCB200_OK)
-    return fail(rc, "invalid parameters");
-  ex.phase(kPhaseGather);
-  {
-    DeviceExec::Scope sc(ex);
-    k_scatter_rows_clip<<<g, 256, 0, ex.stream>>>(dAttrs, dOrder, n, A, clipMax, dAttrsOut);
-    g_launchCount++;
-  }
-  PCC_CUDA_CHECK(cudaGetLastError());
-  return PCCB200_OK;
-}
-
-// one slice, several attributes on the same positions in one pass: one sort,
-// one tree, one dependency chain.  Pointers as in attr_raht_slice, one per set.
-// In two halves, so that the descents of several slices can be issued together
-// (a gang, attr_raht_batch_common): _begin sorts, gathers, builds the tree and
-// either runs the descent or leaves it prepared in ms.defer; _end runs the
-// duplicate tail (if deferred) and scatters the reconstruction back.
-// PCCB200_ERR_UNSUPPORTED: this parameter combination has no fused path.
-struct MultiSlice {
-  int32_t* dOrder = nullptr;
-  int32_t* dAttrs = nullptr;
-  int AT = 0;
-  RahtDeferred<DeviceExec> defer;
-};
-
-int
-attr_raht_slice_multi_begin(DeviceExec& ex, bool forward, const pccb200_raht_params* params,
-                            int numSets, const pccb200_qpset* const* qpsets, const int32_t* dXyz,
-                            const int32_t* const* dAttrsIn, const int* A, int n,
-                            int32_t* const* dCoef, const int64_t* coefStride, MultiSlice& ms,
-                            bool deferDescent)
-{
-  int AT = 0;
-  for (int s = 0; s < numSets; s++)
-    AT += A[s];
-  int64_t* dKeys = ex.alloc<int64_t>(size_t(n));
-  ms.dOrder = ex.alloc<int32_t>(size_t(n));
-  ms.dAttrs = ex.alloc<int32_t>(size_t(n) * AT);
-  ms.AT = AT;
-  device_morton_sort(ex, dXyz, n, dKeys, ms.dOrder);
-  const unsigned g = grid_for(n, ex.numSMs);
-  ex.phase(kPhaseGather);
-  RahtSetIO io[2];
-  for (int s = 0, base = 0; s < numSets; base += A[s], s++) {
-    if (forward) {
-      DeviceExec::Scope sc(ex);
-      k_gather_rows_strided<<<g, 256, 0, ex.stream>>>(dAttrsIn[s], ms.dOrder, n, A[s], ms.dAttrs, AT, base);
-      g_launchCount++;
-    }
-    io[s] = RahtSetIO{qpsets[s], A[s], dCoef[s], coefStride[s]};
-  }
-  int rc = raht_run_sets(ex, *params, numSets, io, forward, dKeys, ms.dAttrs, nullptr, n,
-                         deferDescent ? &ms.defer : nullptr);
-  if (rc != PCCB200_OK)
-    return rc == PCCB200_ERR_UNSUPPORTED ? rc : fail(rc, "invalid parameters");
-  return PCCB200_OK;
-}
-
-void
-attr_raht_slice_multi_end(DeviceExec& ex, int numSets, const int* A, const int* bitdepth, int n,
-                          int32_t* const* dAttrsOut, MultiSlice& ms)
-{
-  if (ms.defer.pending) {
-    ex.phase(kPhaseTail);
-    ex.foreach(ms.defer.nLeaves, ms.defer.tail);
-    ms.defer.pending = false;
-  }
-  const unsigned g = grid_for(n, ex.numSMs);
-  ex.phase(kPhaseGather);
-  for (int s = 0, base = 0; s < numSets; base += A[s], s++) {
-    DeviceExec::Scope sc(ex);
-    k_scatter_rows_clip_strided<<<g, 256, 0, ex.stream>>>(ms.dAttrs, ms.AT, base, ms.dOrder, n, A[s],
-                                                          (1 << bitdepth[s]) - 1, dAttrsOut[s]);
-    g_launchCount++;
-  }
-  PCC_CUDA_CHECK(cudaGetLastError());
-}
-
-int
-attr_raht_slice_multi(DeviceExec& ex, bool forward, const pccb200_raht_params* params,
-                      int numSets, const pccb200_qpset* const* qpsets, const int32_t* dXyz,
-                      const int32_t* const* dAttrsIn, int32_t* const* dAttrsOut, const int* A,
-                      const int* bitdepth, int n, int32_t* const* dCoef, const int64_t* coefStride)
-{
-  MultiSlice ms;
-  int rc = attr_raht_slice_multi_begin(ex, forward, params, numSets, qpsets, dXyz, dAttrsIn, A, n,
-                                       dCoef, coefStride, ms, false);
-  if (rc != PCCB200_OK)
-    return rc;
-  attr_raht_slice_multi_end(ex, numSets, A, bitdepth, n, dAttrsOut, ms);
-  return PCCB200_OK;
-}
-
 int
 check_slices(const void* params, const void* qpset, const void* xyz, const void* attrs,
              const void* coeffs, int A, int bitdepth, const int64_t* sliceOffsets,
@@ -458,68 +342,6 @@ check_slices(const void* params, const void* qpset, const void* xyz, const void*
 }
 
 constexpr int kMaxSliceThreads = 16;
-
-// host pointers: every slice is staged, transformed and returned on its own
-// lane; slices overlap on the device
-int
-attr_raht_common(bool forward, const pccb200_raht_params* params, const pccb200_qpset* qpset,
-                 const int32_t* qpo, const int32_t* xyz, int32_t* attrs, int A,
-                 int bitdepth, const int64_t* sliceOffsets, int numSlices,
-                 int32_t* coeffs)
-{
-  int rc = check_slices(params, qpset, xyz, attrs, coeffs, A, bitdepth, sliceOffsets, numSlices);
-  if (rc != PCCB200_OK)
-    return rc;
-  const int64_t total = sliceOffsets[numSlices];
-  return parallel_for(numSlices, kMaxSliceThreads, [&](int s) -> int {
-    const int64_t o = sliceOffsets[s];
-    const int n = int(sliceOffsets[s + 1] - o);
-    return with_device([&](DeviceExec& ex) -> int {
-      int32_t* dXyz = to_device(ex, xyz + 3 * o, size_t(n) * 3);
-      int32_t* dAttrsIn = forward ? to_device(ex, attrs + o * A, size_t(n) * A) : nullptr;
-      int32_t* dQpoIn = qpo ? to_device(ex, qpo + 2 * o, size_t(n) * 2) : nullptr;
-      int32_t* dCoef = ex.alloc<int32_t>(size_t(n) * A);
-      if (!forward)
-        for (int k = 0; k < A; k++)
-          PCC_CUDA_CHECK(cudaMemcpyAsync(dCoef + size_t(k) * n, coeffs + k * total + o,
-                                         size_t(n) * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                         ex.stream));
-      int32_t* dOut = ex.alloc<int32_t>(size_t(n) * A);
-      int rc2 = attr_raht_slice(ex, forward, params, qpset, dQpoIn, dXyz, dAttrsIn, dOut, A,
-                                bitdepth, n, dCoef, n);
-      if (rc2 != PCCB200_OK)
-        return rc2;
-      to_host(ex, attrs + o * A, dOut, size_t(n) * A);
-      if (forward)
-        for (int k = 0; k < A; k++)
-          to_host(ex, coeffs + k * total + o, dCoef + size_t(k) * n, size_t(n));
-      return PCCB200_OK;
-    });
-  });
-}
-
-int
-attr_raht_common_dev(bool forward, const pccb200_raht_params* params,
-                     const pccb200_qpset* qpset, const int32_t* dQpo, const int32_t* dXyz,
-                     int32_t* dAttrs, int A, int bitdepth, const int64_t* sliceOffsets,
-                     int numSlices, int32_t* dCoef)
-{
-  int rc = check_slices(params, qpset, dXyz, dAttrs, dCoef, A, bitdepth, sliceOffsets, numSlices);
-  if (rc != PCCB200_OK)
-    return rc;
-  const int64_t total = sliceOffsets[numSlices];
-  return parallel_for(numSlices, kMaxSliceThreads, [&](int s) -> int {
-    const int64_t o = sliceOffsets[s];
-    const int n = int(sliceOffsets[s + 1] - o);
-    return with_device([&](DeviceExec& ex) -> int {
-      // in place on the caller's attribute buffer: the gather reads the slice
-      // before the final scatter overwrites it
-      return attr_raht_slice(ex, forward, params, qpset, dQpo ? dQpo + 2 * o : nullptr,
-                             dXyz + 3 * o, dAttrs + o * A, dAttrs + o * A, A, bitdepth, n,
-                             dCoef + o, total);
-    });
-  });
-}
 
 int
 check_multi(const void* params, int numSets, const pccb200_qpset* const* qpsets, const void* xyz,
@@ -541,81 +363,266 @@ check_multi(const void* params, int numSets, const pccb200_qpset* const* qpsets,
   return PCCB200_OK;
 }
 
-// Several attributes of one slice.  Fused pass where the parameters allow it,
-// otherwise one pass per attribute (same results either way).
+// One coding unit of an attribute-RAHT call (a slice, or a whole frame): n
+// points with their positions and optional point qp offsets ([n, 2]), and per
+// attribute set its rows ([n, A], in and out) and coefficient planes
+// (component k at coef + k * coefStride).  dev: device pointers, coded in
+// place; otherwise host pointers.
+struct RahtUnit {
+  int n = 0;
+  const int32_t* xyz = nullptr;
+  const int32_t* qpo = nullptr;
+  bool dev = false;
+  int numSets = 0;
+  const pccb200_qpset* qs[kMaxSets] = {};
+  int A[kMaxSets] = {};
+  int bitdepth[kMaxSets] = {};
+  int32_t* attrs[kMaxSets] = {};
+  int32_t* coef[kMaxSets] = {};
+  int64_t coefStride[kMaxSets] = {};
+
+  RahtUnit only(int s) const  // the same unit with set s alone
+  {
+    RahtUnit u = *this;
+    u.numSets = 1;
+    u.qs[0] = qs[s];
+    u.A[0] = A[s];
+    u.bitdepth[0] = bitdepth[s];
+    u.attrs[0] = attrs[s];
+    u.coef[0] = coef[s];
+    u.coefStride[0] = coefStride[s];
+    return u;
+  }
+};
+
+// Codes a gang of units on one lane.  Each unit in turn is staged in, Morton
+// sorted and gathered, and its tree built with the descent left prepared; the
+// descents of all of them are issued together (WaveDescent::run_gang); then
+// each unit's tail runs, its reconstruction is clipped and scattered back to
+// input order and its results are staged out.
 int
-attr_raht_multi_common(bool forward, bool device, const pccb200_raht_params* params, int numSets,
-                       const pccb200_qpset* const* qpsets, const int32_t* xyz,
-                       int32_t* const* attrs, const int32_t* A, const int32_t* bitdepth, int n,
-                       int32_t* const* coeffs)
+code_units(DeviceExec& ex, bool forward, const pccb200_raht_params& pp, const RahtUnit* units,
+           int m)
+{
+  struct Staged {
+    int32_t* order;
+    int32_t* rows;  // [n, AT]: the components of every set, Morton order
+    int AT;
+    int32_t* out[kMaxSets];
+    int32_t* coef[kMaxSets];
+    int64_t coefStride[kMaxSets];
+    RahtDeferred<DeviceExec> defer;
+  };
+  std::vector<Staged> st(m);
+  for (int i = 0; i < m; i++) {
+    const RahtUnit& u = units[i];
+    Staged& w = st[i];
+    const int n = u.n;
+    const int32_t* dXyz = u.dev ? u.xyz : to_device(ex, u.xyz, size_t(n) * 3);
+    const int32_t* dQpoIn = u.qpo && !u.dev ? to_device(ex, u.qpo, size_t(n) * 2) : u.qpo;
+    const int32_t* dIn[kMaxSets] = {};
+    w.AT = 0;
+    for (int s = 0; s < u.numSets; s++) {
+      const size_t len = size_t(n) * u.A[s];
+      w.AT += u.A[s];
+      if (u.dev) {  // in place: the gather reads the rows before the scatter overwrites them
+        dIn[s] = w.out[s] = u.attrs[s];
+        w.coef[s] = u.coef[s];
+        w.coefStride[s] = u.coefStride[s];
+        continue;
+      }
+      dIn[s] = forward ? to_device(ex, u.attrs[s], len) : nullptr;
+      w.out[s] = ex.alloc<int32_t>(len);
+      w.coef[s] = ex.alloc<int32_t>(len);
+      w.coefStride[s] = n;
+      if (!forward)
+        PCC_CUDA_CHECK(cudaMemcpy2DAsync(w.coef[s], size_t(n) * sizeof(int32_t), u.coef[s],
+                                         size_t(u.coefStride[s]) * sizeof(int32_t),
+                                         size_t(n) * sizeof(int32_t), size_t(u.A[s]),
+                                         cudaMemcpyHostToDevice, ex.stream));
+    }
+    int64_t* dKeys = ex.alloc<int64_t>(size_t(n));
+    w.order = ex.alloc<int32_t>(size_t(n));
+    w.rows = ex.alloc<int32_t>(size_t(n) * w.AT);
+    int32_t* dQpo = dQpoIn ? ex.alloc<int32_t>(size_t(n) * 2) : nullptr;
+    device_morton_sort(ex, dXyz, n, dKeys, w.order);
+    const unsigned g = grid_for(n, ex.numSMs);
+    ex.phase(kPhaseGather);
+    RahtSetIO io[kMaxSets];
+    for (int s = 0, base = 0; s < u.numSets; base += u.A[s], s++) {
+      if (forward) {
+        DeviceExec::Scope sc(ex);
+        k_gather_rows_strided<<<g, 256, 0, ex.stream>>>(dIn[s], w.order, n, u.A[s], w.rows, w.AT,
+                                                        base);
+        g_launchCount++;
+      }
+      io[s] = RahtSetIO{u.qs[s], u.A[s], w.coef[s], w.coefStride[s]};
+    }
+    if (dQpo) {
+      DeviceExec::Scope sc(ex);
+      k_gather_rows_strided<<<g, 256, 0, ex.stream>>>(dQpoIn, w.order, n, 2, dQpo, 2, 0);
+      g_launchCount++;
+    }
+    int rc = raht_run_sets(ex, pp, u.numSets, io, forward, dKeys, w.rows, dQpo, n, &w.defer);
+    if (rc != PCCB200_OK)
+      return fail(rc, "invalid parameters");
+  }
+  std::vector<WaveDescent<DeviceExec>::Job*> jobs;
+  for (Staged& w : st)
+    if (w.defer.pending)
+      jobs.push_back(&w.defer.job);
+  if (!jobs.empty())
+    WaveDescent<DeviceExec>::run_gang(ex, jobs.data(), int(jobs.size()));
+  for (int i = 0; i < m; i++) {
+    const RahtUnit& u = units[i];
+    Staged& w = st[i];
+    const int n = u.n;
+    if (w.defer.pending) {
+      ex.phase(kPhaseTail);
+      ex.foreach(w.defer.nLeaves, w.defer.tail);
+    }
+    const unsigned g = grid_for(n, ex.numSMs);
+    ex.phase(kPhaseGather);
+    for (int s = 0, base = 0; s < u.numSets; base += u.A[s], s++) {
+      DeviceExec::Scope sc(ex);
+      k_scatter_rows_clip_strided<<<g, 256, 0, ex.stream>>>(w.rows, w.AT, base, w.order, n, u.A[s],
+                                                            (1 << u.bitdepth[s]) - 1, w.out[s]);
+      g_launchCount++;
+    }
+    PCC_CUDA_CHECK(cudaGetLastError());
+    if (u.dev)
+      continue;
+    for (int s = 0; s < u.numSets; s++) {
+      to_host(ex, u.attrs[s], w.out[s], size_t(n) * u.A[s]);
+      if (forward)
+        PCC_CUDA_CHECK(cudaMemcpy2DAsync(u.coef[s], size_t(u.coefStride[s]) * sizeof(int32_t),
+                                         w.coef[s], size_t(n) * sizeof(int32_t),
+                                         size_t(n) * sizeof(int32_t), size_t(u.A[s]),
+                                         cudaMemcpyDeviceToHost, ex.stream));
+    }
+  }
+  return PCCB200_OK;
+}
+
+// Validated units, coded on the lanes.  A unit with several attribute sets is
+// coded in one fused pass (one sort, one tree, one dependency chain) where the
+// parameters have one, otherwise as one unit per set; results do not depend
+// on the route.  The units are dealt to the lanes in gangs: a lane prepares
+// the units of its gang in turn and then issues the top-down passes of all of
+// them together, one launch per descent step.  A textured unit keeps only a
+// few warps busy (its blocks form one chain): the number of chains in flight
+// is what the device's throughput follows, and with gangs it is not limited
+// by the number of hardware queues.
+constexpr int kMaxGang = 32;
+constexpr int kBatchLanes = 16;  // lanes a call spreads over (measured: 8, 16 and 32 lanes
+                                 // give the same throughput; fewer lanes = fewer host threads
+                                 // and fewer launches)
+
+int
+code_raht(bool forward, const pccb200_raht_params& pp, const std::vector<RahtUnit>& given)
+{
+  std::vector<RahtUnit> units;
+  for (const RahtUnit& u : given) {
+    bool fuse = u.numSets > 1 && u.n >= 2 && !u.qpo;  // (same test as raht_run_sets)
+    for (int s = 0; s < u.numSets && fuse; s++)
+      fuse = WaveDescent<DeviceExec>::enabled(make_config(pp, *u.qs[s], forward, u.A[s], false));
+    if (fuse || u.numSets == 1)
+      units.push_back(u);
+    else
+      for (int s = 0; s < u.numSets; s++)
+        units.push_back(u.only(s));
+  }
+  const int numUnits = int(units.size());
+  // units per gang: by default the units are spread over all lanes first
+  // (PCCB200_GANG: A/B knob, read per call)
+  const char* eg = getenv("PCCB200_GANG");
+  const int envGang = eg ? atoi(eg) : 0;
+  int gang = envGang > 0 ? envGang : (numUnits + kBatchLanes - 1) / kBatchLanes;
+  gang = gang > kMaxGang ? kMaxGang : gang;
+  const int numGangs = (numUnits + gang - 1) / gang;
+  return parallel_for(numGangs, kMaxLanes, [&](int g) -> int {
+    const int u0 = g * gang;
+    const int m = u0 + gang < numUnits ? gang : numUnits - u0;
+    return with_device([&](DeviceExec& ex) -> int {
+      return code_units(ex, forward, pp, units.data() + u0, m);
+    });
+  });
+}
+
+// one attribute, one unit per slice (coefficients: [A, total] planes)
+int
+attr_raht_slices(bool forward, bool dev, const pccb200_raht_params* params,
+                 const pccb200_qpset* qpset, const int32_t* qpo, const int32_t* xyz,
+                 int32_t* attrs, int A, int bitdepth, const int64_t* sliceOffsets, int numSlices,
+                 int32_t* coeffs)
+{
+  int rc = check_slices(params, qpset, xyz, attrs, coeffs, A, bitdepth, sliceOffsets, numSlices);
+  if (rc != PCCB200_OK)
+    return rc;
+  std::vector<RahtUnit> units(numSlices);
+  for (int s = 0; s < numSlices; s++) {
+    const int64_t o = sliceOffsets[s];
+    RahtUnit& u = units[s];
+    u.n = int(sliceOffsets[s + 1] - o);
+    u.xyz = xyz + 3 * o;
+    u.qpo = qpo ? qpo + 2 * o : nullptr;
+    u.dev = dev;
+    u.numSets = 1;
+    u.qs[0] = qpset;
+    u.A[0] = A;
+    u.bitdepth[0] = bitdepth;
+    u.attrs[0] = attrs + o * A;
+    u.coef[0] = coeffs + o;
+    u.coefStride[0] = sliceOffsets[numSlices];
+  }
+  return code_raht(forward, *params, units);
+}
+
+// several attributes of one unit per xyz[u] (coefficients: [A_s, n[u]] planes);
+// attrs / coeffs hold numSets pointers per unit
+int
+attr_raht_units(bool forward, bool dev, const pccb200_raht_params* params, int numSets,
+                const pccb200_qpset* const* qpsets, int numUnits, const int32_t* const* xyz,
+                int32_t* const* attrs, const int32_t* A, const int32_t* bitdepth,
+                const int32_t* n, int32_t* const* coeffs)
+{
+  std::vector<RahtUnit> units(numUnits);
+  for (int i = 0; i < numUnits; i++) {
+    RahtUnit& u = units[i];
+    u.n = n[i];
+    u.xyz = xyz[i];
+    u.dev = dev;
+    u.numSets = numSets;
+    for (int s = 0; s < numSets; s++) {
+      u.qs[s] = qpsets[s];
+      u.A[s] = A[s];
+      u.bitdepth[s] = bitdepth[s];
+      u.attrs[s] = attrs[size_t(i) * numSets + s];
+      u.coef[s] = coeffs[size_t(i) * numSets + s];
+      u.coefStride[s] = n[i];
+    }
+  }
+  return code_raht(forward, *params, units);
+}
+
+int
+attr_raht_multi(bool forward, bool dev, const pccb200_raht_params* params, int numSets,
+                const pccb200_qpset* const* qpsets, const int32_t* xyz, int32_t* const* attrs,
+                const int32_t* A, const int32_t* bitdepth, int32_t n, int32_t* const* coeffs)
 {
   int rc = check_multi(params, numSets, qpsets, xyz, reinterpret_cast<const void* const*>(attrs),
                        A, bitdepth, reinterpret_cast<const void* const*>(coeffs), n);
   if (rc != PCCB200_OK)
     return rc;
-  rc = with_device([&](DeviceExec& ex) -> int {
-    const int32_t* dXyz = device ? xyz : to_device(ex, xyz, size_t(n) * 3);
-    int32_t* dIn[2];
-    int32_t* dOut[2];
-    int32_t* dCoef[2];
-    int64_t stride[2];
-    for (int s = 0; s < numSets; s++) {
-      stride[s] = n;
-      if (device) {
-        dIn[s] = dOut[s] = attrs[s];
-        dCoef[s] = coeffs[s];
-      } else {
-        dIn[s] = forward ? to_device(ex, attrs[s], size_t(n) * A[s]) : nullptr;
-        dOut[s] = ex.alloc<int32_t>(size_t(n) * A[s]);
-        dCoef[s] = forward ? ex.alloc<int32_t>(size_t(n) * A[s])
-                           : to_device(ex, coeffs[s], size_t(n) * A[s]);
-      }
-    }
-    int rc2 = attr_raht_slice_multi(ex, forward, params, numSets, qpsets, dXyz, dIn, dOut, A,
-                                    bitdepth, n, dCoef, stride);
-    if (rc2 != PCCB200_OK)
-      return rc2;
-    if (!device)
-      for (int s = 0; s < numSets; s++) {
-        to_host(ex, attrs[s], dOut[s], size_t(n) * A[s]);
-        if (forward)
-          to_host(ex, coeffs[s], dCoef[s], size_t(n) * A[s]);
-      }
-    return PCCB200_OK;
-  });
-  if (rc != PCCB200_ERR_UNSUPPORTED)
-    return rc;
-  // no fused path for these parameters: attribute by attribute
-  for (int s = 0; s < numSets; s++) {
-    const int64_t offs[2] = {0, n};
-    rc = device ? attr_raht_common_dev(forward, params, qpsets[s], nullptr, xyz, attrs[s], A[s],
-                                       bitdepth[s], offs, 1, coeffs[s])
-                : attr_raht_common(forward, params, qpsets[s], nullptr, xyz, attrs[s], A[s],
-                                   bitdepth[s], offs, 1, coeffs[s]);
-    if (rc != PCCB200_OK)
-      return rc;
-  }
-  return PCCB200_OK;
+  return attr_raht_units(forward, dev, params, numSets, qpsets, 1, &xyz, attrs, A, bitdepth, &n,
+                         coeffs);
 }
 
-// Many coding units (the slices of a frame, or whole frames: independent
-// point sets, each with the same attributes) in one call.  The units are dealt
-// to the lanes in gangs: a lane sorts / builds the tree of each unit of its
-// gang in turn and then issues the top-down passes of all of them together,
-// one launch per descent step (WaveDescent::run_gang).  A textured unit keeps
-// only a few warps busy (its blocks form one chain): the number of chains in
-// flight is what the device's throughput follows, and with gangs it is no
-// longer limited by the number of hardware queues.
-constexpr int kMaxGang = 32;
-constexpr int kBatchLanes = 16;  // lanes a batch call spreads over (measured: 8, 16 and 32 lanes
-                                 // give the same throughput; fewer lanes = fewer host threads
-                                 // and fewer launches)
-
 int
-attr_raht_batch_common(bool forward, bool device, const pccb200_raht_params* params, int numSets,
-                       const pccb200_qpset* const* qpsets, int numUnits,
-                       const int32_t* const* xyz, int32_t* const* attrs, const int32_t* A,
-                       const int32_t* bitdepth, const int32_t* n, int32_t* const* coeffs)
+attr_raht_batch(bool forward, bool dev, const pccb200_raht_params* params, int numSets,
+                const pccb200_qpset* const* qpsets, int numUnits, const int32_t* const* xyz,
+                int32_t* const* attrs, const int32_t* A, const int32_t* bitdepth,
+                const int32_t* n, int32_t* const* coeffs)
 {
   if (!xyz || !attrs || !coeffs || !n || numUnits <= 0)
     return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
@@ -629,77 +636,8 @@ attr_raht_batch_common(bool forward, bool device, const pccb200_raht_params* par
     if (rc != PCCB200_OK)
       return rc;
   }
-  // the fused pass exists for these parameters?  (same test as raht_run_sets)
-  bool fused = true;
-  if (numSets > 1)
-    for (int u = 0; u < numUnits && fused; u++) {
-      fused = n[u] >= 2;
-      for (int s = 0; s < numSets && fused; s++)
-        fused = WaveDescent<DeviceExec>::enabled(make_config(*params, *qpsets[s], forward, A[s], false));
-    }
-  if (!fused)  // unit by unit, attribute by attribute (results do not depend on the route)
-    return parallel_for(numUnits, kMaxSliceThreads, [&](int u) -> int {
-      return attr_raht_multi_common(forward, device, params, numSets, qpsets, xyz[u],
-                                    attrs + size_t(u) * numSets, A, bitdepth, n[u],
-                                    coeffs + size_t(u) * numSets);
-    });
-  // units per gang: by default the units are spread over all lanes first
-  // (PCCB200_GANG: A/B knob, read per call)
-  const char* eg = getenv("PCCB200_GANG");
-  const int envGang = eg ? atoi(eg) : 0;
-  int gang = envGang > 0 ? envGang : (numUnits + kBatchLanes - 1) / kBatchLanes;
-  gang = gang > kMaxGang ? kMaxGang : gang;
-  const int numGangs = (numUnits + gang - 1) / gang;
-  return parallel_for(numGangs, kMaxLanes, [&](int g) -> int {
-    const int u0 = g * gang;
-    const int u1 = u0 + gang < numUnits ? u0 + gang : numUnits;
-    const int m = u1 - u0;
-    return with_device([&](DeviceExec& ex) -> int {
-      std::vector<MultiSlice> ms(m);
-      std::vector<int32_t*> dOut(size_t(m) * 2), dCoef(size_t(m) * 2);
-      for (int i = 0; i < m; i++) {
-        const int u = u0 + i;
-        const int nu = n[u];
-        const int32_t* dXyz = device ? xyz[u] : to_device(ex, xyz[u], size_t(nu) * 3);
-        int32_t* dIn[2] = {nullptr, nullptr};
-        int64_t stride[2] = {nu, nu};
-        for (int s = 0; s < numSets; s++) {
-          int32_t* a = attrs[size_t(u) * numSets + s];
-          int32_t* c = coeffs[size_t(u) * numSets + s];
-          if (device) {
-            dIn[s] = dOut[2 * i + s] = a;
-            dCoef[2 * i + s] = c;
-          } else {
-            dIn[s] = forward ? to_device(ex, a, size_t(nu) * A[s]) : nullptr;
-            dOut[2 * i + s] = ex.alloc<int32_t>(size_t(nu) * A[s]);
-            dCoef[2 * i + s] = forward ? ex.alloc<int32_t>(size_t(nu) * A[s])
-                                       : to_device(ex, c, size_t(nu) * A[s]);
-          }
-        }
-        int rc2 = attr_raht_slice_multi_begin(ex, forward, params, numSets, qpsets, dXyz, dIn, A, nu,
-                                              &dCoef[2 * i], stride, ms[i], true);
-        if (rc2 != PCCB200_OK)
-          return rc2;
-      }
-      std::vector<WaveDescent<DeviceExec>::Job*> jobs;
-      for (int i = 0; i < m; i++)
-        if (ms[i].defer.pending)
-          jobs.push_back(&ms[i].defer.job);
-      if (!jobs.empty())
-        WaveDescent<DeviceExec>::run_gang(ex, jobs.data(), int(jobs.size()));
-      for (int i = 0; i < m; i++) {
-        const int u = u0 + i;
-        attr_raht_slice_multi_end(ex, numSets, A, bitdepth, n[u], &dOut[2 * i], ms[i]);
-        if (!device)
-          for (int s = 0; s < numSets; s++) {
-            to_host(ex, attrs[size_t(u) * numSets + s], dOut[2 * i + s], size_t(n[u]) * A[s]);
-            if (forward)
-              to_host(ex, coeffs[size_t(u) * numSets + s], dCoef[2 * i + s], size_t(n[u]) * A[s]);
-          }
-      }
-      return PCCB200_OK;
-    });
-  });
+  return attr_raht_units(forward, dev, params, numSets, qpsets, numUnits, xyz, attrs, A, bitdepth,
+                         n, coeffs);
 }
 
 }  // namespace
@@ -819,7 +757,7 @@ pccb200_attr_raht_encode(const pccb200_raht_params* params, const pccb200_qpset*
                          int32_t* coeffs_out)
 {
   const int64_t offs[2] = {0, n};
-  return attr_raht_common(true, params, qpset, point_qp_offsets, xyz, attrs_inout, num_attrs,
+  return attr_raht_slices(true, false, params, qpset, point_qp_offsets, xyz, attrs_inout, num_attrs,
                           bitdepth, offs, 1, coeffs_out);
 }
 
@@ -830,7 +768,7 @@ pccb200_attr_raht_decode(const pccb200_raht_params* params, const pccb200_qpset*
                          const int32_t* coeffs_in)
 {
   const int64_t offs[2] = {0, n};
-  return attr_raht_common(false, params, qpset, point_qp_offsets, xyz, attrs_out, num_attrs,
+  return attr_raht_slices(false, false, params, qpset, point_qp_offsets, xyz, attrs_out, num_attrs,
                           bitdepth, offs, 1, const_cast<int32_t*>(coeffs_in));
 }
 
@@ -841,7 +779,7 @@ pccb200_attr_raht_encode_slices(const pccb200_raht_params* params, const pccb200
                                 const int64_t* slice_offsets, int32_t num_slices,
                                 int32_t* coeffs_out)
 {
-  return attr_raht_common(true, params, qpset, point_qp_offsets, xyz, attrs_inout, num_attrs,
+  return attr_raht_slices(true, false, params, qpset, point_qp_offsets, xyz, attrs_inout, num_attrs,
                           bitdepth, slice_offsets, num_slices, coeffs_out);
 }
 
@@ -853,8 +791,8 @@ pccb200_attr_raht_encode_slices_dev(const pccb200_raht_params* params,
                                     const int64_t* slice_offsets, int32_t num_slices,
                                     int32_t* d_coeffs_out)
 {
-  return attr_raht_common_dev(true, params, qpset, d_point_qp_offsets, d_xyz, d_attrs_inout,
-                              num_attrs, bitdepth, slice_offsets, num_slices, d_coeffs_out);
+  return attr_raht_slices(true, true, params, qpset, d_point_qp_offsets, d_xyz, d_attrs_inout,
+                          num_attrs, bitdepth, slice_offsets, num_slices, d_coeffs_out);
 }
 
 int
@@ -865,9 +803,9 @@ pccb200_attr_raht_decode_slices_dev(const pccb200_raht_params* params,
                                     const int64_t* slice_offsets, int32_t num_slices,
                                     const int32_t* d_coeffs_in)
 {
-  return attr_raht_common_dev(false, params, qpset, d_point_qp_offsets, d_xyz, d_attrs_out,
-                              num_attrs, bitdepth, slice_offsets, num_slices,
-                              const_cast<int32_t*>(d_coeffs_in));
+  return attr_raht_slices(false, true, params, qpset, d_point_qp_offsets, d_xyz, d_attrs_out,
+                          num_attrs, bitdepth, slice_offsets, num_slices,
+                          const_cast<int32_t*>(d_coeffs_in));
 }
 
 int
@@ -876,8 +814,8 @@ pccb200_attr_raht_encode_multi(const pccb200_raht_params* params, int32_t num_se
                                int32_t* const* attrs_inout, const int32_t* num_attrs,
                                const int32_t* bitdepths, int32_t n, int32_t* const* coeffs_out)
 {
-  return attr_raht_multi_common(true, false, params, num_sets, qpsets, xyz, attrs_inout,
-                                num_attrs, bitdepths, n, coeffs_out);
+  return attr_raht_multi(true, false, params, num_sets, qpsets, xyz, attrs_inout,
+                         num_attrs, bitdepths, n, coeffs_out);
 }
 
 int
@@ -887,9 +825,9 @@ pccb200_attr_raht_decode_multi(const pccb200_raht_params* params, int32_t num_se
                                const int32_t* bitdepths, int32_t n,
                                const int32_t* const* coeffs_in)
 {
-  return attr_raht_multi_common(false, false, params, num_sets, qpsets, xyz, attrs_out,
-                                num_attrs, bitdepths, n,
-                                const_cast<int32_t* const*>(coeffs_in));
+  return attr_raht_multi(false, false, params, num_sets, qpsets, xyz, attrs_out,
+                         num_attrs, bitdepths, n,
+                         const_cast<int32_t* const*>(coeffs_in));
 }
 
 int
@@ -899,8 +837,8 @@ pccb200_attr_raht_encode_multi_dev(const pccb200_raht_params* params, int32_t nu
                                    const int32_t* bitdepths, int32_t n,
                                    int32_t* const* d_coeffs_out)
 {
-  return attr_raht_multi_common(true, true, params, num_sets, qpsets, d_xyz, d_attrs_inout,
-                                num_attrs, bitdepths, n, d_coeffs_out);
+  return attr_raht_multi(true, true, params, num_sets, qpsets, d_xyz, d_attrs_inout,
+                         num_attrs, bitdepths, n, d_coeffs_out);
 }
 
 int
@@ -910,9 +848,9 @@ pccb200_attr_raht_decode_multi_dev(const pccb200_raht_params* params, int32_t nu
                                    const int32_t* bitdepths, int32_t n,
                                    const int32_t* const* d_coeffs_in)
 {
-  return attr_raht_multi_common(false, true, params, num_sets, qpsets, d_xyz, d_attrs_out,
-                                num_attrs, bitdepths, n,
-                                const_cast<int32_t* const*>(d_coeffs_in));
+  return attr_raht_multi(false, true, params, num_sets, qpsets, d_xyz, d_attrs_out,
+                         num_attrs, bitdepths, n,
+                         const_cast<int32_t* const*>(d_coeffs_in));
 }
 
 int
@@ -922,8 +860,8 @@ pccb200_attr_raht_encode_multi_batch(const pccb200_raht_params* params, int32_t 
                                      const int32_t* num_attrs, const int32_t* bitdepths,
                                      const int32_t* n, int32_t* const* coeffs_out)
 {
-  return attr_raht_batch_common(true, false, params, num_sets, qpsets, num_units, xyz,
-                                attrs_inout, num_attrs, bitdepths, n, coeffs_out);
+  return attr_raht_batch(true, false, params, num_sets, qpsets, num_units, xyz,
+                         attrs_inout, num_attrs, bitdepths, n, coeffs_out);
 }
 
 int
@@ -933,8 +871,8 @@ pccb200_attr_raht_decode_multi_batch(const pccb200_raht_params* params, int32_t 
                                      const int32_t* num_attrs, const int32_t* bitdepths,
                                      const int32_t* n, const int32_t* const* coeffs_in)
 {
-  return attr_raht_batch_common(false, false, params, num_sets, qpsets, num_units, xyz, attrs_out,
-                                num_attrs, bitdepths, n, const_cast<int32_t* const*>(coeffs_in));
+  return attr_raht_batch(false, false, params, num_sets, qpsets, num_units, xyz, attrs_out,
+                         num_attrs, bitdepths, n, const_cast<int32_t* const*>(coeffs_in));
 }
 
 int
@@ -945,8 +883,8 @@ pccb200_attr_raht_encode_multi_batch_dev(const pccb200_raht_params* params, int3
                                          const int32_t* bitdepths, const int32_t* n,
                                          int32_t* const* d_coeffs_out)
 {
-  return attr_raht_batch_common(true, true, params, num_sets, qpsets, num_units, d_xyz,
-                                d_attrs_inout, num_attrs, bitdepths, n, d_coeffs_out);
+  return attr_raht_batch(true, true, params, num_sets, qpsets, num_units, d_xyz,
+                         d_attrs_inout, num_attrs, bitdepths, n, d_coeffs_out);
 }
 
 int
@@ -956,9 +894,9 @@ pccb200_attr_raht_decode_multi_batch_dev(const pccb200_raht_params* params, int3
                                          const int32_t* num_attrs, const int32_t* bitdepths,
                                          const int32_t* n, const int32_t* const* d_coeffs_in)
 {
-  return attr_raht_batch_common(false, true, params, num_sets, qpsets, num_units, d_xyz,
-                                d_attrs_out, num_attrs, bitdepths, n,
-                                const_cast<int32_t* const*>(d_coeffs_in));
+  return attr_raht_batch(false, true, params, num_sets, qpsets, num_units, d_xyz,
+                         d_attrs_out, num_attrs, bitdepths, n,
+                         const_cast<int32_t* const*>(d_coeffs_in));
 }
 
 
@@ -1599,16 +1537,24 @@ pccb200_attr_raht_encode_symbols(const pccb200_raht_params* params, const pccb20
     return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
   return with_device([&](DeviceExec& ex) -> int {
     const int A = num_attrs;
-    int32_t* dXyz = to_device(ex, xyz, size_t(n) * 3);
-    int32_t* dAttrsIn = to_device(ex, attrs_inout, size_t(n) * A);
-    int32_t* dQpoIn = point_qp_offsets ? to_device(ex, point_qp_offsets, size_t(n) * 2) : nullptr;
-    int32_t* dCoef = ex.alloc<int32_t>(size_t(n) * A);
-    int32_t* dOut = ex.alloc<int32_t>(size_t(n) * A);
-    int rc2 = attr_raht_slice(ex, true, params, qpset, dQpoIn, dXyz, dAttrsIn, dOut, A, bitdepth,
-                              n, dCoef, n);
+    // the unit is staged here: its coefficients stay on the device
+    RahtUnit u;
+    u.n = n;
+    u.xyz = to_device(ex, xyz, size_t(n) * 3);
+    u.qpo = point_qp_offsets ? to_device(ex, point_qp_offsets, size_t(n) * 2) : nullptr;
+    u.dev = true;
+    u.numSets = 1;
+    u.qs[0] = qpset;
+    u.A[0] = A;
+    u.bitdepth[0] = bitdepth;
+    u.attrs[0] = to_device(ex, attrs_inout, size_t(n) * A);
+    u.coef[0] = ex.alloc<int32_t>(size_t(n) * A);
+    u.coefStride[0] = n;
+    int rc2 = code_units(ex, true, *params, &u, 1);
     if (rc2 != PCCB200_OK)
       return rc2;
-    to_host(ex, attrs_inout, dOut, size_t(n) * A);
+    const int32_t* dCoef = u.coef[0];
+    to_host(ex, attrs_inout, u.attrs[0], size_t(n) * A);
     int32_t* dRuns = ex.alloc<int32_t>(size_t(n));
     int32_t* dValues = ex.alloc<int32_t>(size_t(n) * A);
     uint8_t* dCtx = ex.alloc<uint8_t>(size_t(n));

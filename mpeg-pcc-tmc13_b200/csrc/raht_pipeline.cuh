@@ -18,7 +18,11 @@
 //                                           *total (executor memory) = count
 //   void subsample_distance(SubsampleDistanceFn fn, int nCells)   (lod_pipeline.cuh)
 //   void block_stage(BlockFn fn, int64_t nBlocks, int* tzNext)
-//                                           one top-down stage; see exec_cuda.cuh
+//                                           one top-down stage with the
+//                                           thread-per-block body, then the
+//                                           zero-run counter to tzNext;
+//                                           the stages of a descent WaveDescent
+//                                           (below) does not take
 //
 // Mirrors the control flow of uraht_process (tmc3/RAHT.cpp:977-1976).
 #pragma once
@@ -146,7 +150,6 @@ struct RahtSetRt {
   const QpTables* qt;
   int32_t* coef;
   int64_t coefStride;
-  int* tz;  // zero-run words of the set (layout: tzOff), or null
 };
 
 // A call whose descent and tail have been prepared but not run yet: the
@@ -167,7 +170,9 @@ struct RahtDeferred {
 // attributes coded on the same positions in one pass: they share the tree and
 // every geometry-only step; that needs the executor's own descent
 // (WaveDescent) and returns PCCB200_ERR_UNSUPPORTED where it cannot be used
-// (the caller then codes the attributes one by one).  Returns a PCCB200_* status.
+// (the caller codes such attributes one by one).  With defer, a descent
+// WaveDescent runs is left prepared in *defer (pending) together with the
+// tail; everything else runs here.  Returns a PCCB200_* status.
 template<class Exec>
 int
 raht_run_sets(Exec& ex, const pccb200_raht_params& pp, int numSets, const RahtSetIO* io,
@@ -289,9 +294,23 @@ raht_run_sets(Exec& ex, const pccb200_raht_params& pp, int numSets, const RahtSe
   //-- descent, coarse to fine
   ex.phase(2);  // block transform
   int qpLayer = 0;
-  if (hasStages) {
-    // zero-run look-back words: a region of (blocks + 1) words per stage;
-    // word 0 of a region is the counter handed over by the previous stage
+  bool descended = false;
+  if constexpr (WaveDescent<Exec>::available) {
+    if (hasStages && (numSets > 1 || WaveDescent<Exec>::enabled(cfg))) {
+      typename WaveDescent<Exec>::Job local;
+      typename WaveDescent<Exec>::Job* job = defer ? &defer->job : &local;
+      WaveDescent<Exec>::prepare(ex, cfg, numSets, rt, stages, *job);
+      if (defer)
+        defer->pending = true;
+      else
+        WaveDescent<Exec>::run_gang(ex, &job, 1);
+      descended = true;
+    }
+  }
+  if (hasStages && !descended) {
+    // one set (several need WaveDescent).  Zero-run look-back words: a region
+    // of (blocks + 1) words per stage; word 0 of a region is the counter
+    // handed over by the previous stage
     const bool rdoq = forward && !cfg.haar;
     std::vector<int64_t> tzOff(stages.size() + 1, 0);
     int* tz = nullptr;
@@ -302,30 +321,14 @@ raht_run_sets(Exec& ex, const pccb200_raht_params& pp, int numSets, const RahtSe
         total += (si == int(stages.size()) - 1 ? 1 : stages[si + 1].n) + 1;
       }
       total++;
-      tz = ex.template alloc<int>(size_t(total) * numSets);
-      ex.zero(tz, size_t(total) * numSets * sizeof(int));
+      tz = ex.template alloc<int>(size_t(total));
+      ex.zero(tz, size_t(total) * sizeof(int));
       int init = tz_pack(kTzExit, 0);
-      for (int s = 0; s < numSets; s++) {
-        rt[s].tz = tz + size_t(total) * s;
-        ex.upload(rt[s].tz + tzOff[stages.size() - 1], &init, sizeof(int));
-      }
-    }
-
-    bool descended = false;
-    if constexpr (WaveDescent<Exec>::available) {
-      if (numSets > 1 || WaveDescent<Exec>::enabled(cfg)) {
-        if (defer) {
-          WaveDescent<Exec>::prepare(ex, cfg, numSets, rt, stages, tzOff, defer->job);
-          defer->pending = true;
-        } else {
-          WaveDescent<Exec>::run(ex, cfg, numSets, rt, stages, tzOff);
-        }
-        descended = true;
-      }
+      ex.upload(tz + tzOff[stages.size() - 1], &init, sizeof(int));
     }
 
     int acLayer = -1;
-    for (int si = int(stages.size()) - 1; si >= 0 && !descended; si--) {
+    for (int si = int(stages.size()) - 1; si >= 0; si--) {
       qpLayer = qpLayer + 1 < qs.num_layers ? qpLayer + 1 : qs.num_layers - 1;
       acLayer++;
       BlockFn fn;

@@ -139,14 +139,6 @@ struct WaveDescent<DeviceExec> {
 
   static bool enabled(const RahtConfig& cfg)
   {
-    static const int mode = [] {
-      const char* e = getenv("PCCB200_BLOCK_KERNEL");
-      if (!e)
-        return 0;
-      return !strcmp(e, "thread") ? 1 : !strcmp(e, "warp") ? 2 : 0;
-    }();
-    if (mode)
-      return false;
     // AC-coefficient qp offsets in the encoder keep the exact-counter protocol
     // of the thread-per-block body (see DeviceExec::block_stage)
     if (cfg.isEncoder && !cfg.haar && cfg.numAcLayers > 0)
@@ -157,12 +149,13 @@ struct WaveDescent<DeviceExec> {
   // Everything one unit's descent needs between its preparation (geometry,
   // schedule: steps 1-3) and its stage launches (step 4).  Kept so that the
   // stage launches of several units can be issued together (run_gang).
+  // stages[0] = leaves ... stages.back() = children of the root block;
+  // rt: the attributes coded in this pass (cfg.A = all their components).
   struct Job {
     RahtConfig cfg;
     int numSets = 0;
     RahtSetRt rt[kMaxSets];
     std::vector<Stage> stages;
-    std::vector<int64_t> tzOff;
     int top = 0;
     bool rdoq = false;
     std::vector<WarpBlockArgs> args;   // one per descent step, [0] = root block
@@ -174,30 +167,11 @@ struct WaveDescent<DeviceExec> {
     TzRegion* dRegions[kMaxSets] = {nullptr, nullptr};
   };
 
-  // stages[0] = leaves ... stages.back() = children of the root block.
-  // rt: the attributes coded in this pass (cfg.A = all their components);
-  // rt[s].tz / tzOff: zero-run words as laid out by raht_run_sets.
-  static void run(DeviceExec& ex, const RahtConfig& cfg, int numSets, const RahtSetRt* rt,
-                  const std::vector<Stage>& stages, const std::vector<int64_t>& tzOff)
-  {
-    Job job;
-    prepare(ex, cfg, numSets, rt, stages, tzOff, job);
-    ex.phase(kPhaseBlock);
-    for (int d = 0; d <= job.top; d++) {
-      const int nBlocks = stage_prep(ex, job, d);
-      {
-        DeviceExec::Scope sc(ex);
-        k_block_warp<<<unsigned(ex.block_grid(nBlocks)), kWarpBlockThreads, 0, ex.stream>>>(
-          job.args[d], job.tickets + d);
-        g_launchCount++;
-      }
-      PCC_CUDA_CHECK(cudaGetLastError());
-    }
-  }
-
-  // The stage launches of several prepared units, step by step: launch d
-  // carries descent step d of every unit that has one (units are independent;
-  // a step needs only the previous step of its own unit).
+  // The stage launches of prepared units, step by step: launch d carries
+  // descent step d of every unit that has one (units are independent; a step
+  // needs only the previous step of its own unit).  A step of one unit runs
+  // k_block_warp with the unit's arguments as its kernel parameter; a step of
+  // several runs k_block_warp_gang over a table of their arguments.
   static void run_gang(DeviceExec& ex, Job* const* jobs, int numJobs)
   {
     int maxTop = -1;
@@ -217,8 +191,11 @@ struct WaveDescent<DeviceExec> {
         tab.push_back(GangEntry{job.args[d], job.tickets + d});
       }
       const int units = int(tab.size());
-      GangEntry* dTab = ex.alloc<GangEntry>(tab.size());
-      ex.upload(dTab, tab.data(), tab.size() * sizeof(GangEntry));
+      GangEntry* dTab = nullptr;
+      if (units > 1) {
+        dTab = ex.alloc<GangEntry>(tab.size());
+        ex.upload(dTab, tab.data(), tab.size() * sizeof(GangEntry));
+      }
       // the lane's share of the machine, divided among the units of the gang
       int64_t perUnit = ex.block_grid(int64_t(1) << 40) / units;
       const int64_t useful = (int64_t(maxBlocks) + kWarpBlockThreads / 32 - 1) / (kWarpBlockThreads / 32);
@@ -229,7 +206,11 @@ struct WaveDescent<DeviceExec> {
       perUnit = perUnit < 1 ? 1 : perUnit;
       {
         DeviceExec::Scope sc(ex);
-        k_block_warp_gang<<<unsigned(perUnit * units), kWarpBlockThreads, 0, ex.stream>>>(dTab, units);
+        if (units == 1)
+          k_block_warp<<<unsigned(perUnit), kWarpBlockThreads, 0, ex.stream>>>(tab[0].a,
+                                                                                tab[0].ticket);
+        else
+          k_block_warp_gang<<<unsigned(perUnit * units), kWarpBlockThreads, 0, ex.stream>>>(dTab, units);
         g_launchCount++;
       }
       PCC_CUDA_CHECK(cudaGetLastError());
@@ -238,7 +219,7 @@ struct WaveDescent<DeviceExec> {
 
   // steps 1-3 (nothing here reads an attribute value)
   static void prepare(DeviceExec& ex, const RahtConfig& cfg, int numSets, const RahtSetRt* rt,
-                      const std::vector<Stage>& stages, const std::vector<int64_t>& tzOff, Job& job)
+                      const std::vector<Stage>& stages, Job& job)
   {
     const int top = int(stages.size()) - 1;
     const bool rdoq = cfg.isEncoder && !cfg.haar;
@@ -247,16 +228,11 @@ struct WaveDescent<DeviceExec> {
     for (int s = 0; s < numSets; s++)
       job.rt[s] = rt[s];
     job.stages = stages;
-    job.tzOff = tzOff;
     job.top = top;
     job.rdoq = rdoq;
     const char* ep = getenv("PCCB200_POLL_NS");  // A/B knob, read per call
     const int pollNs = ep ? atoi(ep) : 32;
-    static const bool mortonOrder = [] {  // A/B: coding order everywhere
-      const char* e = getenv("PCCB200_WAVE_ORDER");
-      return e && !strcmp(e, "morton");
-    }();
-    const bool wave = cfg.predictionEnabled && cfg.subnode && !rdoq && !mortonOrder;
+    const bool wave = cfg.predictionEnabled && cfg.subnode && !rdoq;
 
     //-- row space: one segment per descent step below the root
     LevelArgs la = {};
