@@ -493,7 +493,10 @@ struct DeviceExec {
   {
     static const int perSM = [] {
       int v = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_block_warp, kWarpBlockThreads, 0)
+      // (the generic variant: the leaner ones may fit more CTAs per SM, but more
+      // resident warps per SM measured slower -- see below)
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_block_warp_gang<kBlockGeneric>,
+                                                        kWarpBlockThreads, 0)
           != cudaSuccess)
         v = 0;
       return v < 1 ? 1 : v;

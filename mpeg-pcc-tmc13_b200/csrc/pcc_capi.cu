@@ -1108,6 +1108,28 @@ pccb200_profile_read(double ms_out[PCCB200_NUM_PHASES], uint64_t launches_out[PC
   }
 }
 
+#ifdef PCCB200_HOP_STATS
+// Developer build only (make hopstats; tools/hop_profile.py): the block
+// kernel's cycle counters, kHopCounters values per descent step, read after a
+// device synchronise and cleared.  Returns the number of values per step.
+extern "C" int
+pccb200_hop_stats_read(uint64_t* out, int32_t steps)
+{
+  static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "counter type");
+  unsigned long long host[pccb200::kHopStages][pccb200::kHopCounters];
+  if (cudaDeviceSynchronize() != cudaSuccess
+      || cudaMemcpyFromSymbol(host, pccb200::g_hopStats, sizeof(host)) != cudaSuccess)
+    return -1;
+  for (int s = 0; s < steps && s < pccb200::kHopStages; s++)
+    for (int c = 0; c < pccb200::kHopCounters; c++)
+      out[size_t(s) * pccb200::kHopCounters + c] = host[s][c];
+  memset(host, 0, sizeof(host));
+  if (cudaMemcpyToSymbol(pccb200::g_hopStats, host, sizeof(host)) != cudaSuccess)
+    return -1;
+  return pccb200::kHopCounters;
+}
+#endif
+
 int
 pccb200_lod_build(const pccb200_lod_params* params, const int32_t* xyz, int32_t n,
                   pccb200_predictor* preds_out, uint32_t* indexes_out,

@@ -327,6 +327,52 @@ zero_run_rate(int tz)
   return 11 + 2 * a - 1 + 2;
 }
 
+// RDOQ classification of a coefficient, 6 bits; eight of them, in scan order,
+// make the list a block of the warp kernel publishes (raht_block_warp.cuh):
+//   0      all components quantise to zero: never resets the run
+//   1      RDOQ removes it whatever the run length: never resets either
+//   2      always resets the run (sum |q| >= 3, or RDOQ never fires)
+//   3..8   removed if the run before it is at least 1,2,3,5,7,9 long
+//   8 + a  removed if the run before it is at least 10 + 2^(a-1), a = 1..30
+constexpr int kCodeZero = 0;
+constexpr int kCodeRemoved = 1;
+constexpr int kCodeHard = 2;
+
+// The smallest zero-run length tz for which the reference's test
+// (RAHT.cpp:1617-1636)
+//     (Dist2 << 26) < lambda * (Rate(tz) + ((Ratecoeff + 128) >> 8))
+// holds, as a code.  Rate(tz) (zero_run_rate) is a non-decreasing step
+// function taking 37 values: 1,2,3,5,7,9,11 (tz = 0,1,2,3,5,7,9) and 12 + 2a
+// (tz = 10 + 2^(a-1), a = 1..30), so with rc = (Ratecoeff + 128) >> 8 the
+// answer is the first of them that is >= floor(lhs / lambda) + 1 - rc.  The
+// quotient is below 72 + rc once the test is known to hold for the largest
+// rate: a float estimate (invLambda = 1.0f / float(lambda), which depends on
+// the quantiser alone and is prepared ahead of the values the block waits
+// for) is within one of it, and one 64-bit product settles which.  Dist2 << 26
+// wraps like the 64-bit shift it stands for; lambda * (72 + rc) must not
+// (lambda is a squared quantiser step times 25 or 35).
+PCC_HD int
+rdoq_code(int64_t dist2, int64_t lambda, float invLambda, int rateCoeff)
+{
+  const int64_t lhs = int64_t(uint64_t(dist2) << 26);
+  const int rc = (rateCoeff + 128) >> 8;
+  if (lhs >= lambda * (72 + rc))
+    return kCodeHard;
+  if (lhs < lambda)  // (a wrapped, negative left side included)
+    return kCodeRemoved;
+  int q = int(float(lhs) * invLambda);
+  const int64_t prod = lambda * q;
+  if (prod > lhs)
+    q--;
+  else if (prod + lambda <= lhs)
+    q++;
+  const int need = q + 1 - rc;  // the smallest rate for which the test holds
+  // index of the first rate >= need: 0..6 for need <= 11, then rate(i) = 2i
+  const int idx = need <= 1 ? 0 : need <= 11 ? int((0x66554433210ull >> (4 * (need - 1))) & 15u)
+                                             : need <= 14 ? 7 : (need + 1) >> 1;
+  return idx == 0 ? kCodeRemoved : 2 + idx;
+}
+
 PCC_TABLE(int16_t, kLutLog, 16,
           {0, 256, 406, 512, 594, 662, 719, 768, 812, 850, 886, 918, 947, 975, 1000, 1024})
 PCC_HD int

@@ -204,17 +204,34 @@ struct WaveDescent<DeviceExec> {
       if (ec && atoi(ec) > 0 && perUnit > atoi(ec))
         perUnit = atoi(ec);
       perUnit = perUnit < 1 ? 1 : perUnit;
+      // the variant every unit of the launch can run (raht_block_warp.cuh)
+      BlockVariant variant = block_variant(tab[0].a);
+      for (int u = 1; u < units; u++)
+        if (block_variant(tab[u].a) != variant)
+          variant = kBlockGeneric;
       {
         DeviceExec::Scope sc(ex);
-        if (units == 1)
-          k_block_warp<<<unsigned(perUnit), kWarpBlockThreads, 0, ex.stream>>>(tab[0].a,
-                                                                                tab[0].ticket);
+        if (variant == kBlockRdoq2)
+          launch_blocks<kBlockRdoq2>(ex, tab, dTab, perUnit);
+        else if (variant == kBlockRdoq1)
+          launch_blocks<kBlockRdoq1>(ex, tab, dTab, perUnit);
         else
-          k_block_warp_gang<<<unsigned(perUnit * units), kWarpBlockThreads, 0, ex.stream>>>(dTab, units);
+          launch_blocks<kBlockGeneric>(ex, tab, dTab, perUnit);
         g_launchCount++;
       }
       PCC_CUDA_CHECK(cudaGetLastError());
     }
+  }
+
+  template<BlockVariant V>
+  static void launch_blocks(DeviceExec& ex, const std::vector<GangEntry>& tab, const GangEntry* dTab,
+                            int64_t perUnit)
+  {
+    const int units = int(tab.size());
+    if (units == 1)
+      k_block_warp<V><<<unsigned(perUnit), kWarpBlockThreads, 0, ex.stream>>>(tab[0].a, tab[0].ticket);
+    else
+      k_block_warp_gang<V><<<unsigned(perUnit * units), kWarpBlockThreads, 0, ex.stream>>>(dTab, units);
   }
 
   // steps 1-3 (nothing here reads an attribute value)
