@@ -350,6 +350,80 @@ int pccb200_recolour(const pccb200_recolour_params* params, const int32_t* sourc
                      const int32_t* target_xyz, int32_t n_target, int32_t bitdepth,
                      int32_t* target_attrs_out);
 
+/* Several attribute sets of a slice in one call, and many slices or frames --
+ *
+ * The encoder recolours every attribute of a slice onto the same coded
+ * positions (tmc3/encoder.cpp:1031-1037 calls recolour() once per attribute;
+ * recolourColour and recolourReflectance, tmc3/pointset_processing.cpp:253-958,
+ * each build both kd-trees and run both searches).  None of that depends on the
+ * attribute values, so these entries do it once per unit: both grid hashes,
+ * the forward and backward k-nearest-neighbour searches, the backward lists
+ * and their sort.  The forward and final colours of all num_sets sets (1 to
+ * PCCB200_MAX_RECOLOUR_SETS) are then computed together, one launch each; a
+ * call launches as many kernels for two sets as for one.  Each set's output is
+ * bit-identical to one pccb200_recolour call per set, and so to the oracle.
+ *
+ *   source_attrs[s] (n_source x num_attrs[s]), num_attrs[s] (1 or 3),
+ *   bitdepths[s] (1..16), target_attrs_out[s] (n_target x num_attrs[s])
+ *   describe set s.
+ *
+ * The *_batch entries take num_units units (the slices of a frame, or whole
+ * frames): source_xyz[u] (n_source[u] x 3), target_xyz[u] (n_target[u] x 3),
+ * source_attrs[u * num_sets + s] and target_attrs_out[u * num_sets + s] as
+ * above.  Scale and offset are per unit (source_to_target_scale[u],
+ * tgt_to_src_offsets[3 * u .. 3 * u + 2]) because the slices of a frame differ
+ * in their origin (_sliceOrigin).  Units are spread over the library's lanes;
+ * results are bit-identical to one pccb200_recolour_multi call per unit.
+ *
+ * The *_dev entries take device pointers for positions and attributes; the
+ * pointer arrays, num_attrs, bitdepths, scales and offsets stay host arrays.
+ * The stream-ordering note of the RAHT *_dev entries applies.
+ *
+ * Arguments are checked before a device is looked up; every malformed one
+ * returns PCCB200_ERR_INVALID_ARG.  A coordinate outside [0, 2^21) is found on
+ * the device: PCCB200_ERR_INVALID_ARG, and pccb200_last_error() names the unit.
+ *
+ * Workspace of a unit in flight, with kf = num_neighbours_fwd, kb =
+ * num_neighbours_bwd and SA = the sum of num_attrs[s]: 36 + 24 kb bytes per
+ * source point and 44 + 12 kf + 4 SA bytes per target point, plus 12 bytes per
+ * point and cell-size attempt of each grid's sort (usually two to four
+ * attempts); the host-pointer entries add 12 + 4 SA bytes per point on either
+ * side for the staged copies.  With the defaults (8 / 1 neighbours) and colour
+ * plus reflectance: about 0.2 KB per target point and 0.1 KB per source point. */
+#define PCCB200_MAX_RECOLOUR_SETS 4
+int pccb200_recolour_multi(const pccb200_recolour_params* params, int32_t num_sets,
+                           const int32_t* source_xyz, int32_t n_source,
+                           const int32_t* const* source_attrs, const int32_t* num_attrs,
+                           const int32_t* bitdepths, double source_to_target_scale,
+                           const int32_t tgt_to_src_offset[3],
+                           const int32_t* target_xyz, int32_t n_target,
+                           int32_t* const* target_attrs_out);
+int pccb200_recolour_multi_dev(const pccb200_recolour_params* params, int32_t num_sets,
+                               const int32_t* d_source_xyz, int32_t n_source,
+                               const int32_t* const* d_source_attrs, const int32_t* num_attrs,
+                               const int32_t* bitdepths, double source_to_target_scale,
+                               const int32_t tgt_to_src_offset[3],
+                               const int32_t* d_target_xyz, int32_t n_target,
+                               int32_t* const* d_target_attrs_out);
+int pccb200_recolour_multi_batch(const pccb200_recolour_params* params, int32_t num_sets,
+                                 int32_t num_units,
+                                 const int32_t* const* source_xyz, const int32_t* n_source,
+                                 const int32_t* const* source_attrs,
+                                 const int32_t* num_attrs, const int32_t* bitdepths,
+                                 const double* source_to_target_scale,
+                                 const int32_t* tgt_to_src_offsets,
+                                 const int32_t* const* target_xyz, const int32_t* n_target,
+                                 int32_t* const* target_attrs_out);
+int pccb200_recolour_multi_batch_dev(const pccb200_recolour_params* params, int32_t num_sets,
+                                     int32_t num_units,
+                                     const int32_t* const* d_source_xyz, const int32_t* n_source,
+                                     const int32_t* const* d_source_attrs,
+                                     const int32_t* num_attrs, const int32_t* bitdepths,
+                                     const double* source_to_target_scale,
+                                     const int32_t* tgt_to_src_offsets,
+                                     const int32_t* const* d_target_xyz, const int32_t* n_target,
+                                     int32_t* const* d_target_attrs_out);
+
 /* Per-phase device timing (CUDA events around every kernel launch on
  * the call's stream).  Phases: 0 Morton keys + radix sort, 1 tree build
  * (histogram, compaction, leaf / merge kernels), 2 block transform (the

@@ -11,6 +11,8 @@
 // passes and deals the units to lanes, code_units codes a gang of them on one
 // lane.  The attribute-lifting entries (single, slices, a level-of-detail
 // handle; host or device pointers) share code_lift, one LiftUnit per lane.
+// The recolouring entries (one or several attribute sets, one unit or a batch;
+// host or device pointers) share code_recolour, one RecolourUnit per lane.
 #include <cuda_runtime.h>
 
 #include <stdlib.h>
@@ -772,6 +774,108 @@ attr_lift(bool forward, bool dev, const pccb200_lod_params* lod, pccb200_lod_han
     u.handle = h;
   }
   return code_lift(forward, *qpset, lcpEnabled != 0, A, bitdepth, units);
+}
+
+// One unit of a recolouring call (a slice, or a whole frame): source and
+// target positions, scale and offset, and per attribute set its source values,
+// component count, bit depth and output (sets[s].refined1 is not used here).
+// dev: device pointers; otherwise host pointers.
+struct RecolourUnit {
+  int nSrc = 0, nTgt = 0;
+  const int32_t* srcXyz = nullptr;
+  const int32_t* tgtXyz = nullptr;
+  double scale = 1.0;
+  int32_t off[3] = {};
+  bool dev = false;
+  int numSets = 0;
+  RecolourSet sets[kRecolourMaxSets] = {};
+};
+
+// Validated units over at most kCallLanes lanes, one lane each: stage in,
+// recolour_run, stage out.  nameUnits: a failure's message names the unit.
+int
+code_recolour(const pccb200_recolour_params& rp, const std::vector<RecolourUnit>& units,
+              bool nameUnits)
+{
+  return parallel_for(int(units.size()), kCallLanes, [&](int i) -> int {
+    const RecolourUnit& u = units[i];
+    return with_device([&](DeviceExec& ex) -> int {
+      RecolourSet sets[kRecolourMaxSets];
+      const int32_t* dSrc = u.dev ? u.srcXyz : to_device(ex, u.srcXyz, size_t(u.nSrc) * 3);
+      for (int s = 0; s < u.numSets; s++) {
+        sets[s] = u.sets[s];
+        if (!u.dev)
+          sets[s].srcAttr = to_device(ex, u.sets[s].srcAttr, size_t(u.nSrc) * u.sets[s].A);
+      }
+      const int32_t* dTgt = u.dev ? u.tgtXyz : to_device(ex, u.tgtXyz, size_t(u.nTgt) * 3);
+      for (int s = 0; s < u.numSets && !u.dev; s++)
+        sets[s].out = ex.alloc<int32_t>(size_t(u.nTgt) * u.sets[s].A);
+      int rc = recolour_run(ex, rp, dSrc, u.nSrc, u.scale, u.off, dTgt, u.nTgt, u.numSets, sets);
+      if (rc != PCCB200_OK)
+        return fail(rc, (nameUnits ? "unit " + std::to_string(i) + ": " : std::string())
+                          + "invalid recolouring parameters (neighbour counts, scale, or a "
+                            "coordinate outside [0, 2^21))");
+      for (int s = 0; s < u.numSets && !u.dev; s++)
+        to_host(ex, u.sets[s].out, sets[s].out, size_t(u.nTgt) * u.sets[s].A);
+      return PCCB200_OK;
+    });
+  });
+}
+
+// Checks the arguments of a pccb200_recolour_multi* call, before any device is
+// looked up, and describes its units.  Unit u: srcXyz[u], tgtXyz[u], scale[u],
+// offsets[3u..3u+2], and per set s srcAttrs[u * numSets + s], out[u * numSets + s].
+int
+recolour_units(bool dev, const pccb200_recolour_params* params, int numSets, int numUnits,
+               const int32_t* const* srcXyz, const int32_t* nSrc,
+               const int32_t* const* srcAttrs, const int32_t* A, const int32_t* bitdepth,
+               const double* scale, const int32_t* offsets, const int32_t* const* tgtXyz,
+               const int32_t* nTgt, int32_t* const* out, std::vector<RecolourUnit>& units)
+{
+  if (!params || !srcXyz || !nSrc || !srcAttrs || !A || !bitdepth || !scale || !offsets
+      || !tgtXyz || !nTgt || !out || numUnits <= 0 || numSets < 1 || numSets > kRecolourMaxSets)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  units.resize(numUnits);
+  for (int i = 0; i < numUnits; i++) {
+    RecolourUnit& u = units[i];
+    u.nSrc = nSrc[i];
+    u.nTgt = nTgt[i];
+    u.srcXyz = srcXyz[i];
+    u.tgtXyz = tgtXyz[i];
+    u.scale = scale[i];
+    for (int k = 0; k < 3; k++)
+      u.off[k] = offsets[3 * size_t(i) + k];
+    u.dev = dev;
+    u.numSets = numSets;
+    bool null = !u.srcXyz || !u.tgtXyz;
+    for (int s = 0; s < numSets; s++) {
+      const size_t at = size_t(i) * numSets + s;
+      u.sets[s] = RecolourSet{srcAttrs[at], A[s], bitdepth[s], nullptr, out[at]};
+      null = null || !srcAttrs[at] || !out[at];
+    }
+    if (null)
+      return fail(PCCB200_ERR_INVALID_ARG, "unit " + std::to_string(i) + ": null pointer");
+    if (!recolour_args_valid(*params, u.nSrc, u.nTgt, u.scale, numSets, u.sets))
+      return fail(PCCB200_ERR_INVALID_ARG,
+                  "unit " + std::to_string(i) + ": bad point count, neighbour count, component "
+                  "count, bit depth, search range or scale");
+  }
+  return PCCB200_OK;
+}
+
+int
+recolour_multi(bool dev, const pccb200_recolour_params* params, int numSets, int numUnits,
+               const int32_t* const* srcXyz, const int32_t* nSrc,
+               const int32_t* const* srcAttrs, const int32_t* A, const int32_t* bitdepth,
+               const double* scale, const int32_t* offsets, const int32_t* const* tgtXyz,
+               const int32_t* nTgt, int32_t* const* out)
+{
+  std::vector<RecolourUnit> units;
+  int rc = recolour_units(dev, params, numSets, numUnits, srcXyz, nSrc, srcAttrs, A, bitdepth,
+                          scale, offsets, tgtXyz, nTgt, out, units);
+  if (rc != PCCB200_OK)
+    return rc;
+  return code_recolour(*params, units, true);
 }
 
 }  // namespace
@@ -1685,19 +1789,74 @@ pccb200_recolour(const pccb200_recolour_params* params, const int32_t* source_xy
   if (!params || !source_xyz || !source_attrs || !tgt_to_src_offset || !target_xyz
       || !target_attrs_out || n_source <= 0 || n_target <= 0 || (num_attrs != 1 && num_attrs != 3))
     return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
-  return with_device([&](DeviceExec& ex) -> int {
-    int32_t* dSrc = to_device(ex, source_xyz, size_t(n_source) * 3);
-    int32_t* dAttr = to_device(ex, source_attrs, size_t(n_source) * num_attrs);
-    int32_t* dTgt = to_device(ex, target_xyz, size_t(n_target) * 3);
-    int32_t* dOut = ex.alloc<int32_t>(size_t(n_target) * num_attrs);
-    int rc = recolour_run(ex, *params, dSrc, dAttr, num_attrs, n_source, source_to_target_scale,
-                          tgt_to_src_offset, dTgt, n_target, bitdepth, dOut);
-    if (rc != PCCB200_OK)
-      return fail(rc, "invalid recolouring parameters (neighbour counts, scale, or a coordinate "
-                      "outside [0, 2^21))");
-    to_host(ex, target_attrs_out, dOut, size_t(n_target) * num_attrs);
-    return PCCB200_OK;
-  });
+  // the other ranges are checked on the device path (recolour_run)
+  std::vector<RecolourUnit> units(1);
+  RecolourUnit& u = units[0];
+  u.nSrc = n_source;
+  u.nTgt = n_target;
+  u.srcXyz = source_xyz;
+  u.tgtXyz = target_xyz;
+  u.scale = source_to_target_scale;
+  for (int k = 0; k < 3; k++)
+    u.off[k] = tgt_to_src_offset[k];
+  u.numSets = 1;
+  u.sets[0] = RecolourSet{source_attrs, num_attrs, bitdepth, nullptr, target_attrs_out};
+  return code_recolour(*params, units, false);
+}
+
+int
+pccb200_recolour_multi(const pccb200_recolour_params* params, int32_t num_sets,
+                       const int32_t* source_xyz, int32_t n_source,
+                       const int32_t* const* source_attrs, const int32_t* num_attrs,
+                       const int32_t* bitdepths, double source_to_target_scale,
+                       const int32_t tgt_to_src_offset[3], const int32_t* target_xyz,
+                       int32_t n_target, int32_t* const* target_attrs_out)
+{
+  return recolour_multi(false, params, num_sets, 1, &source_xyz, &n_source, source_attrs,
+                        num_attrs, bitdepths, &source_to_target_scale, tgt_to_src_offset,
+                        &target_xyz, &n_target, target_attrs_out);
+}
+
+int
+pccb200_recolour_multi_dev(const pccb200_recolour_params* params, int32_t num_sets,
+                           const int32_t* d_source_xyz, int32_t n_source,
+                           const int32_t* const* d_source_attrs, const int32_t* num_attrs,
+                           const int32_t* bitdepths, double source_to_target_scale,
+                           const int32_t tgt_to_src_offset[3], const int32_t* d_target_xyz,
+                           int32_t n_target, int32_t* const* d_target_attrs_out)
+{
+  return recolour_multi(true, params, num_sets, 1, &d_source_xyz, &n_source, d_source_attrs,
+                        num_attrs, bitdepths, &source_to_target_scale, tgt_to_src_offset,
+                        &d_target_xyz, &n_target, d_target_attrs_out);
+}
+
+int
+pccb200_recolour_multi_batch(const pccb200_recolour_params* params, int32_t num_sets,
+                             int32_t num_units, const int32_t* const* source_xyz,
+                             const int32_t* n_source, const int32_t* const* source_attrs,
+                             const int32_t* num_attrs, const int32_t* bitdepths,
+                             const double* source_to_target_scale,
+                             const int32_t* tgt_to_src_offsets, const int32_t* const* target_xyz,
+                             const int32_t* n_target, int32_t* const* target_attrs_out)
+{
+  return recolour_multi(false, params, num_sets, num_units, source_xyz, n_source, source_attrs,
+                        num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
+                        target_xyz, n_target, target_attrs_out);
+}
+
+int
+pccb200_recolour_multi_batch_dev(const pccb200_recolour_params* params, int32_t num_sets,
+                                 int32_t num_units, const int32_t* const* d_source_xyz,
+                                 const int32_t* n_source, const int32_t* const* d_source_attrs,
+                                 const int32_t* num_attrs, const int32_t* bitdepths,
+                                 const double* source_to_target_scale,
+                                 const int32_t* tgt_to_src_offsets,
+                                 const int32_t* const* d_target_xyz, const int32_t* n_target,
+                                 int32_t* const* d_target_attrs_out)
+{
+  return recolour_multi(true, params, num_sets, num_units, d_source_xyz, n_source, d_source_attrs,
+                        num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
+                        d_target_xyz, n_target, d_target_attrs_out);
 }
 
 }  // extern "C"

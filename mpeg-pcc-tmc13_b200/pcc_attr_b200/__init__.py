@@ -98,7 +98,8 @@ EXPORTS = [
     "pccb200_profile_reset", "pccb200_quant_weights", "pccb200_quant_weights_fixed",
     "pccb200_quant_weights_scalable", "pccb200_raht_forward", "pccb200_raht_inverse",
     "pccb200_raht_params_default", "pccb200_raht_set_prediction_weights", "pccb200_recolour",
-    "pccb200_recolour_params_default", "pccb200_set_device",
+    "pccb200_recolour_multi", "pccb200_recolour_multi_batch", "pccb200_recolour_multi_batch_dev",
+    "pccb200_recolour_multi_dev", "pccb200_recolour_params_default", "pccb200_set_device",
     "pccb200_time_begin", "pccb200_time_end", "pccb200_xyz_to_rpl",
 ]
 NUM_PHASES = 8
@@ -400,6 +401,71 @@ def recolour(params, source_xyz, source_attrs, target_xyz, scale=1.0, offset=(0,
                                   C.c_int32(sx.shape[0]), C.c_double(scale), off, _p(tx, C.c_int32),
                                   C.c_int32(tx.shape[0]), C.c_int32(bitdepth), _p(out, C.c_int32)))
     return out
+
+
+def _recolour_batch_args(sources, source_attrs, targets, scales, offsets, outs, bitdepths, ptr):
+    """C arrays of a pccb200_recolour_multi_batch(_dev) call; source_attrs[u][s], outs[u][s]"""
+    m, k = len(sources), len(source_attrs[0])
+    VP = C.c_void_p * m
+    AP = C.c_void_p * (m * k)
+    return (C.c_int32(k), C.c_int32(m), VP(*[ptr(x) for x in sources]),
+            (C.c_int32 * m)(*[int(x.shape[0]) for x in sources]),
+            AP(*[ptr(a) for u in source_attrs for a in u]),
+            (C.c_int32 * k)(*[int(a.shape[1]) for a in source_attrs[0]]),
+            (C.c_int32 * k)(*bitdepths), (C.c_double * m)(*[float(s) for s in scales]),
+            (C.c_int32 * (3 * m))(*[int(v) for o in offsets for v in o]),
+            VP(*[ptr(x) for x in targets]), (C.c_int32 * m)(*[int(x.shape[0]) for x in targets]),
+            AP(*[ptr(o) for u in outs for o in u]))
+
+
+def recolour_multi(params, source_xyz, source_attrs, target_xyz, scale=1.0, offset=(0, 0, 0),
+                   bitdepths=None):
+    """several attribute sets on the same positions in one call
+    (pccb200_recolour_multi); source_attrs[s]: [n_source, A_s] -> [[n_target, A_s] int32]"""
+    sx = np.ascontiguousarray(source_xyz, dtype=np.int32)
+    tx = np.ascontiguousarray(target_xyz, dtype=np.int32)
+    sa = [np.ascontiguousarray(a, dtype=np.int32).reshape(sx.shape[0], -1) for a in source_attrs]
+    k = len(sa)
+    outs = [np.zeros((tx.shape[0], a.shape[1]), dtype=np.int32) for a in sa]
+    IP = C.POINTER(C.c_int32) * k
+    _check(lib().pccb200_recolour_multi(
+        C.byref(params), C.c_int32(k), _p(sx, C.c_int32), C.c_int32(sx.shape[0]),
+        IP(*[_p(a, C.c_int32) for a in sa]), (C.c_int32 * k)(*[a.shape[1] for a in sa]),
+        (C.c_int32 * k)(*(bitdepths or [8] * k)), C.c_double(scale),
+        (C.c_int32 * 3)(*[int(v) for v in offset]), _p(tx, C.c_int32), C.c_int32(tx.shape[0]),
+        IP(*[_p(o, C.c_int32) for o in outs])))
+    return outs
+
+
+def recolour_multi_batch(params, sources, source_attrs, targets, scales, offsets, bitdepths=None):
+    """many units (slices / frames) in one call (pccb200_recolour_multi_batch):
+    sources[u] [n_source_u, 3], source_attrs[u][s] [n_source_u, A_s], targets[u],
+    scales[u], offsets[u] (3) -> outs[u][s] [n_target_u, A_s] int32"""
+    sources = [np.ascontiguousarray(x, dtype=np.int32) for x in sources]
+    targets = [np.ascontiguousarray(x, dtype=np.int32) for x in targets]
+    sa = [[np.ascontiguousarray(a, dtype=np.int32).reshape(x.shape[0], -1) for a in u]
+          for x, u in zip(sources, source_attrs)]
+    outs = [[np.zeros((t.shape[0], a.shape[1]), dtype=np.int32) for a in u] for t, u in zip(targets, sa)]
+    k = len(sa[0])
+    args = _recolour_batch_args(sources, sa, targets, scales, offsets, outs, bitdepths or [8] * k,
+                                lambda x: x.ctypes.data)
+    _check(lib().pccb200_recolour_multi_batch(C.byref(params), *args))
+    return outs
+
+
+def recolour_multi_batch_dev(params, sources, source_attrs, targets, scales, offsets, outs,
+                             bitdepths=None):
+    """as recolour_multi_batch with contiguous int32 torch CUDA tensors (device
+    pointers); the results are written into outs[u][s] [n_target_u, A_s].  The
+    producing stream must be synchronised before the call (see the header)."""
+    tensors = list(sources) + list(targets) + [a for u in source_attrs for a in u] + [o for u in outs for o in u]
+    for t in tensors:
+        if not (t.is_cuda and t.is_contiguous() and str(t.dtype) == "torch.int32"):
+            raise PccB200Error("recolour_multi_batch_dev takes contiguous int32 CUDA tensors")
+    k = len(source_attrs[0])
+    args = _recolour_batch_args(sources, source_attrs, targets, scales, offsets, outs,
+                                bitdepths or [8] * k, lambda x: x.data_ptr())
+    _check(lib().pccb200_recolour_multi_batch_dev(C.byref(params), *args))
 
 
 def quant_weights(preds, num_points_in_lod):
