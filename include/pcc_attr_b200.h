@@ -624,6 +624,113 @@ int pccb200_attr_lift_decode_lod(pccb200_lod_handle handle, const pccb200_qpset*
                                  int32_t* attrs_out, int32_t num_attrs, int32_t bitdepth,
                                  const int32_t* values_in, const int8_t* lcp_coeffs);
 
+/* Several attributes of one slice in ONE lifting pass ---------------------------
+ *
+ * For attributes that share the positions and the LoD parameters of a slice --
+ * the case where the reference reuses _lods for the next attribute
+ * (AttributeLods::isReusable) -- these entries build the levels of detail and
+ * the quantisation weights once, and run the forward and inverse lifting
+ * passes once over the components of all num_sets sets (1 to
+ * PCCB200_MAX_LIFT_SETS) side by side: a call makes the lifting-pass launches
+ * of one attribute whatever the number of sets.  Each set keeps its own QpSet,
+ * last-component prediction, bit-depth clip and outputs, and its results are
+ * bit-identical to one pccb200_attr_lift_encode / _decode call per set.
+ * Attributes whose LoD parameters differ need separate calls.  Per-point qp
+ * offsets are not taken here (use the one-attribute entries).
+ *
+ *   qpsets[s], lcp_enabled[s], attrs[s] (n x num_attrs[s], point order; in and
+ *   out when encoding, out when decoding), num_attrs[s] (1 or 3), bitdepths[s]
+ *   (1..16), values[s] (n x num_attrs[s], coding order) and lcp_coeffs[s] (a
+ *   host row of PCCB200_MAX_LODS entries, num_detail_levels of them used)
+ *   describe set s.  lcp_coeffs[s] may be NULL where the set does not use it
+ *   (the decoder needs it for a three-component set with lcp_enabled; the
+ *   encoder writes it when given), and lcp_coeffs itself may be NULL when no
+ *   set does.
+ *
+ * The *_batch entries take num_units units (the slices of a frame, or whole
+ * frames), each with its own LoD parameters lods[u] (dist2 is set per slice,
+ * abh.attr_dist2_delta), positions xyz[u] (n[u] x 3) and per set
+ * attrs[u * num_sets + s], values[u * num_sets + s] and
+ * lcp_coeffs[u * num_sets + s]; qpsets, lcp_enabled, num_attrs and bitdepths
+ * are per set.  Units are spread over the library's lanes; results are
+ * bit-identical to one *_multi call per unit.
+ *
+ * The *_dev entries take device pointers for positions, attributes and values;
+ * the pointer arrays, the lcp rows and every per-set scalar stay on the host.
+ * The stream-ordering note of the RAHT *_dev entries applies.
+ *
+ * Arguments are checked before a device is looked up; every malformed one
+ * returns PCCB200_ERR_INVALID_ARG, and pccb200_last_error() names the unit or
+ * the set.  Predictors that reference their own level of detail return
+ * PCCB200_ERR_UNSUPPORTED, as the one-attribute entries do.
+ *
+ * Workspace of a unit in flight, with SA = the sum of num_attrs[s].  This is
+ * an estimate summed from the per-point allocations of the LoD build, the
+ * predictors, the quantisation weights and the lifting coefficients; it has not
+ * been measured.  About 160 bytes per point for the levels of detail and the
+ * quantisation weights (plus 4 ceil(log2 n) with centroid decimation, and the
+ * grid-cell tables), and at most 8 + 16 SA for the lifting.  The host-pointer
+ * entries add 12 + 12 SA for the staged copies.  Colour plus reflectance: about
+ * 0.23 KB per point, 0.29 KB with host pointers. */
+#define PCCB200_MAX_LIFT_SETS 4
+int pccb200_attr_lift_encode_multi(const pccb200_lod_params* lod, int32_t num_sets,
+                                   const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                   const int32_t* xyz, int32_t n, int32_t* const* attrs_inout,
+                                   const int32_t* num_attrs, const int32_t* bitdepths,
+                                   int32_t* const* values_out, int8_t* const* lcp_coeffs_out);
+int pccb200_attr_lift_decode_multi(const pccb200_lod_params* lod, int32_t num_sets,
+                                   const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                   const int32_t* xyz, int32_t n, int32_t* const* attrs_out,
+                                   const int32_t* num_attrs, const int32_t* bitdepths,
+                                   const int32_t* const* values_in,
+                                   const int8_t* const* lcp_coeffs);
+int pccb200_attr_lift_encode_multi_dev(const pccb200_lod_params* lod, int32_t num_sets,
+                                       const pccb200_qpset* const* qpsets,
+                                       const int32_t* lcp_enabled, const int32_t* d_xyz,
+                                       int32_t n, int32_t* const* d_attrs_inout,
+                                       const int32_t* num_attrs, const int32_t* bitdepths,
+                                       int32_t* const* d_values_out,
+                                       int8_t* const* lcp_coeffs_out);
+int pccb200_attr_lift_decode_multi_dev(const pccb200_lod_params* lod, int32_t num_sets,
+                                       const pccb200_qpset* const* qpsets,
+                                       const int32_t* lcp_enabled, const int32_t* d_xyz,
+                                       int32_t n, int32_t* const* d_attrs_out,
+                                       const int32_t* num_attrs, const int32_t* bitdepths,
+                                       const int32_t* const* d_values_in,
+                                       const int8_t* const* lcp_coeffs);
+int pccb200_attr_lift_encode_multi_batch(int32_t num_units, const pccb200_lod_params* const* lods,
+                                         int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                         const int32_t* lcp_enabled, const int32_t* const* xyz,
+                                         const int32_t* n, int32_t* const* attrs_inout,
+                                         const int32_t* num_attrs, const int32_t* bitdepths,
+                                         int32_t* const* values_out,
+                                         int8_t* const* lcp_coeffs_out);
+int pccb200_attr_lift_decode_multi_batch(int32_t num_units, const pccb200_lod_params* const* lods,
+                                         int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                         const int32_t* lcp_enabled, const int32_t* const* xyz,
+                                         const int32_t* n, int32_t* const* attrs_out,
+                                         const int32_t* num_attrs, const int32_t* bitdepths,
+                                         const int32_t* const* values_in,
+                                         const int8_t* const* lcp_coeffs);
+int pccb200_attr_lift_encode_multi_batch_dev(int32_t num_units,
+                                             const pccb200_lod_params* const* lods,
+                                             int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                             const int32_t* lcp_enabled,
+                                             const int32_t* const* d_xyz, const int32_t* n,
+                                             int32_t* const* d_attrs_inout,
+                                             const int32_t* num_attrs, const int32_t* bitdepths,
+                                             int32_t* const* d_values_out,
+                                             int8_t* const* lcp_coeffs_out);
+int pccb200_attr_lift_decode_multi_batch_dev(int32_t num_units,
+                                             const pccb200_lod_params* const* lods,
+                                             int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                             const int32_t* lcp_enabled,
+                                             const int32_t* const* d_xyz, const int32_t* n,
+                                             int32_t* const* d_attrs_out,
+                                             const int32_t* num_attrs, const int32_t* bitdepths,
+                                             const int32_t* const* d_values_in,
+                                             const int8_t* const* lcp_coeffs);
+
 /* ---------------------------------------------------------------------------
  * Spherical coordinates for attribute coding of LiDAR slices (the step before
  * the attribute transforms when attr_aps.spherical_coord_flag is set). */

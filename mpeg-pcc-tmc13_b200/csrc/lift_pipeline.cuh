@@ -47,6 +47,77 @@ lod_state_build(Exec& ex, const pccb200_lod_params& lod, const int32_t* xyz, int
   return run_quant_weights(ex, st.preds, n, st.npl, st.lodCount, st.qw);
 }
 
+// One attribute set of a lifting call: what is coded per attribute on shared
+// levels of detail.  attrsIn [n*A] (encoder) and attrsOut [n*A]
+// (reconstruction): point order, executor memory; they may alias.  values
+// [n*A]: coding order, executor memory (out when forward).  lcp: host array of
+// PCCB200_MAX_LODS + 1 entries (computed when forward, read otherwise; used
+// with A == 3 and lcpEnabled only).
+constexpr int kLiftMaxSets = 4;
+
+struct LiftSet {
+  int A;          // 1 or 3
+  int bitdepth;   // 1..16
+  const pccb200_qpset* qpset;
+  bool lcpEnabled;
+  const int32_t* attrsIn;
+  int32_t* attrsOut;
+  int32_t* values;
+  int8_t* lcp;
+};
+
+// 1..kLiftMaxSets attribute sets on prepared levels of detail (the case where
+// the reference reuses _lods for the next attribute).  The sets' components
+// are gathered side by side into one row per point (SA = the sum of their A),
+// so the forward and inverse lifting passes run once for all of them, with the
+// launches of one set; gather, quantisation (own QpSet, own last-component
+// prediction) and the clipped write-back are launched once per set.  Each
+// set's results are bit-identical to a call with that set alone.  qpoIn
+// [n*2] or null: point order, executor memory, applies to every set.
+template<class Exec>
+int
+attr_lift_on_lods(Exec& ex, bool forward, const LodState& st, const int32_t* qpoIn, int numSets,
+                  const LiftSet* sets)
+{
+  if (numSets < 1 || numSets > kLiftMaxSets)
+    return PCCB200_ERR_INVALID_ARG;
+  int SA = 0;
+  for (int s = 0; s < numSets; s++) {
+    if (sets[s].A != 1 && sets[s].A != 3)
+      return PCCB200_ERR_INVALID_ARG;
+    SA += sets[s].A;
+  }
+  const int n = st.n;
+  int64_t* coef = ex.template alloc<int64_t>(size_t(n) * SA);
+  int32_t* qpo = nullptr;
+  if (qpoIn) {
+    qpo = ex.template alloc<int32_t>(size_t(n) * 2);
+    ex.foreach(n, GatherQpoFn{qpoIn, st.idx, qpo});
+  }
+  int rc;
+  if (forward) {
+    for (int s = 0, off = 0; s < numSets; off += sets[s].A, s++)
+      ex.foreach(n, GatherAttrShiftFn{sets[s].attrsIn, st.idx, sets[s].A, SA, off, coef});
+    rc = run_lift(ex, true, st.preds, st.qw, n, st.npl, st.lodCount, coef, SA);
+    if (rc != PCCB200_OK)
+      return rc;
+  }
+  for (int s = 0, off = 0; s < numSets; off += sets[s].A, s++) {
+    const LiftSet& t = sets[s];
+    rc = run_lift_quant(ex, forward, *t.qpset, qpo, st.qw, n, st.npl, st.lodCount,
+                        st.numDetailLevels, coef, SA, off, t.A, t.lcpEnabled, t.lcp, t.values);
+    if (rc != PCCB200_OK)
+      return rc;
+  }
+  rc = run_lift(ex, false, st.preds, st.qw, n, st.npl, st.lodCount, coef, SA);
+  if (rc != PCCB200_OK)
+    return rc;
+  for (int s = 0, off = 0; s < numSets; off += sets[s].A, s++)
+    ex.foreach(n, ScatterReconFn{coef, st.idx, sets[s].A, SA, off, (1 << sets[s].bitdepth) - 1,
+                                 sets[s].attrsOut});
+  return PCCB200_OK;
+}
+
 // One attribute on prepared levels of detail.  attrsIn [n*A] (encoder),
 // qpoIn [n*2] or null: point order, executor memory.  values [n*A]: coding
 // order (out when forward).  attrsOut [n*A]: reconstruction in point order.
@@ -57,29 +128,24 @@ attr_lift_on_lods(Exec& ex, bool forward, const LodState& st, const pccb200_qpse
                   bool lcpEnabled, const int32_t* qpoIn, const int32_t* attrsIn,
                   int32_t* attrsOut, int A, int bitdepth, int32_t* values, int8_t* lcp)
 {
-  const int n = st.n;
-  int64_t* coef = ex.template alloc<int64_t>(size_t(n) * A);
-  int32_t* qpo = nullptr;
-  if (qpoIn) {
-    qpo = ex.template alloc<int32_t>(size_t(n) * 2);
-    ex.foreach(n, GatherQpoFn{qpoIn, st.idx, qpo});
-  }
-  int rc;
-  if (forward) {
-    ex.foreach(n, GatherAttrShiftFn{attrsIn, st.idx, A, coef});
-    rc = run_lift(ex, true, st.preds, st.qw, n, st.npl, st.lodCount, coef, A);
-    if (rc != PCCB200_OK)
-      return rc;
-  }
-  rc = run_lift_quant(ex, forward, qpset, qpo, st.qw, n, st.npl, st.lodCount, st.numDetailLevels,
-                      coef, A, lcpEnabled, lcp, values);
+  const LiftSet set{A, bitdepth, &qpset, lcpEnabled, attrsIn, attrsOut, values, lcp};
+  return attr_lift_on_lods(ex, forward, st, qpoIn, 1, &set);
+}
+
+// Levels of detail of xyz [n*3] (executor memory), then attr_lift_on_lods.
+template<class Exec>
+int
+attr_lift_run(Exec& ex, bool forward, const pccb200_lod_params& lod, const int32_t* qpoIn,
+              const int32_t* xyz, int n, int numSets, const LiftSet* sets)
+{
+  LodState st;
+  st.preds = ex.template alloc<pccb200_predictor>(n);
+  st.idx = ex.template alloc<uint32_t>(n);
+  st.qw = ex.template alloc<uint64_t>(n);
+  int rc = lod_state_build(ex, lod, xyz, n, st);
   if (rc != PCCB200_OK)
     return rc;
-  rc = run_lift(ex, false, st.preds, st.qw, n, st.npl, st.lodCount, coef, A);
-  if (rc != PCCB200_OK)
-    return rc;
-  ex.foreach(n, ScatterReconFn{coef, st.idx, A, (1 << bitdepth) - 1, attrsOut});
-  return PCCB200_OK;
+  return attr_lift_on_lods(ex, forward, st, qpoIn, numSets, sets);
 }
 
 // xyz [n*3], attrsIn [n*A] (encoder), qpoIn [n*2] or null: point order,
@@ -92,15 +158,8 @@ attr_lift_run(Exec& ex, bool forward, const pccb200_lod_params& lod, const pccb2
               bool lcpEnabled, const int32_t* qpoIn, const int32_t* xyz, const int32_t* attrsIn,
               int32_t* attrsOut, int A, int n, int bitdepth, int32_t* values, int8_t* lcp)
 {
-  LodState st;
-  st.preds = ex.template alloc<pccb200_predictor>(n);
-  st.idx = ex.template alloc<uint32_t>(n);
-  st.qw = ex.template alloc<uint64_t>(n);
-  int rc = lod_state_build(ex, lod, xyz, n, st);
-  if (rc != PCCB200_OK)
-    return rc;
-  return attr_lift_on_lods(ex, forward, st, qpset, lcpEnabled, qpoIn, attrsIn, attrsOut, A,
-                           bitdepth, values, lcp);
+  const LiftSet set{A, bitdepth, &qpset, lcpEnabled, attrsIn, attrsOut, values, lcp};
+  return attr_lift_run(ex, forward, lod, qpoIn, xyz, n, 1, &set);
 }
 
 }  // namespace pccb200

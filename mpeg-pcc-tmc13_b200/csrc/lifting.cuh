@@ -203,12 +203,14 @@ struct LodTable {
 // per-LoD sums for computeLastComponentPredictionCoeff (note the reference's
 // truncation of the products to int)
 struct LcpSumFn {
-  const int64_t* coeffs;  // n*3
+  const int64_t* coeffs;  // row i at coeffs + i * stride + off, 3 components
+  int stride, off;
   LodTable lt;
   uint64_t* sums;  // [lod][2]: sum k1*k2, sum k1*k1 (two's complement)
   PCC_HD void operator()(int64_t i) const
   {
-    const uint64_t k1 = uint64_t(coeffs[i * 3 + 1]), k2 = uint64_t(coeffs[i * 3 + 2]);
+    const int64_t* c = &coeffs[i * stride + off];
+    const uint64_t k1 = uint64_t(c[1]), k2 = uint64_t(c[2]);
     const int32_t m12 = int32_t(uint32_t(k1 * k2));
     const int32_t m11 = int32_t(uint32_t(k1 * k1));
     const int l = lt.lod_of(i);
@@ -237,13 +239,14 @@ struct LcpSumFn {
 struct LiftQuantFn {
   int forward;
   int A;
+  int stride, off;  // coefficient row i at attrs + i * stride + off
   LayerQp layers[PCCB200_MAX_QP_LAYERS];
   int numLayers;
   LodTable lt;
   int lcp[PCCB200_MAX_LODS + 1];
   const int32_t* qpo;      // n*2 in predictor order, or null
   const uint64_t* qw;
-  int64_t* attrs;          // n*A coefficients in / reconstructed coefficients out
+  int64_t* attrs;          // coefficients in / reconstructed coefficients out
   int32_t* values;         // n*A quantised values (out when forward, in otherwise)
   PCC_HD void operator()(int64_t i) const
   {
@@ -253,7 +256,7 @@ struct LiftQuantFn {
     make_quantizers(layers[layer], qpo ? qpo[2 * i] : 0, qpo ? qpo[2 * i + 1] : 0, q);
     const int64_t iqw = int64_t(irsqrt64(qw[i]));
     const int64_t qwt = int64_t((qw[i] * uint64_t(iqw) + (uint64_t(1) << 39)) >> 40);
-    int64_t* a = &attrs[i * A];
+    int64_t* a = &attrs[i * stride + off];
     int32_t* v = &values[i * A];
     if (forward)
       v[0] = int32_t(q[0].quantize(a[0] * qwt));
@@ -293,24 +296,28 @@ lcp_from_sums(const int64_t* sums, int lodCount, int numDetailLevels, int8_t* ou
     out[lod] = lod ? out[lod - 1] : 0;
 }
 
-// attrs: n*A coefficients (executor memory).  lcpInOut: host array of
-// numDetailLevels entries; computed when forward && lcpEnabled, read when
-// !forward && lcpEnabled.
+// attrs: A coefficients per point at attrs + i * stride + off (executor
+// memory; stride = A, off = 0 for one attribute, or one attribute's columns of
+// rows holding several).  lcpInOut: host array of numDetailLevels entries;
+// computed when forward && lcpEnabled, read when !forward && lcpEnabled.
 template<class Exec>
 int
 run_lift_quant(Exec& ex, bool forward, const pccb200_qpset& qs, const int32_t* qpo,
                const uint64_t* qw, int64_t n, const uint32_t* numPointsInLod, int lodCount,
-               int numDetailLevels, int64_t* attrs, int A, bool lcpEnabled, int8_t* lcpInOut,
-               int32_t* values)
+               int numDetailLevels, int64_t* attrs, int stride, int off, int A, bool lcpEnabled,
+               int8_t* lcpInOut, int32_t* values)
 {
   if (lodCount < 1 || lodCount > PCCB200_MAX_LODS || numDetailLevels < lodCount
       || numDetailLevels > PCCB200_MAX_LODS || qs.num_layers < 1
-      || qs.num_layers > PCCB200_MAX_QP_LAYERS || (A != 1 && A != 3))
+      || qs.num_layers > PCCB200_MAX_QP_LAYERS || (A != 1 && A != 3) || off < 0
+      || off + A > stride)
     return PCCB200_ERR_INVALID_ARG;
   ex.phase(5);
   LiftQuantFn fn;
   fn.forward = forward;
   fn.A = A;
+  fn.stride = stride;
+  fn.off = off;
   fn.numLayers = qs.num_layers;
   for (int i = 0; i < qs.num_layers; i++) {
     fn.layers[i].luma = qs.layers[i][0];
@@ -335,7 +342,7 @@ run_lift_quant(Exec& ex, bool forward, const pccb200_qpset& qs, const int32_t* q
     if (forward) {
       uint64_t* dSums = ex.template alloc<uint64_t>(2 * PCCB200_MAX_LODS + 2);
       ex.zero(dSums, (2 * PCCB200_MAX_LODS + 2) * sizeof(uint64_t));
-      ex.foreach(n, LcpSumFn{attrs, fn.lt, dSums});
+      ex.foreach(n, LcpSumFn{attrs, stride, off, fn.lt, dSums});
       int64_t sums[2 * PCCB200_MAX_LODS + 2];
       ex.download(sums, dSums, sizeof(sums));
       lcp_from_sums(sums, effCount, numDetailLevels, lcpInOut);
@@ -352,16 +359,19 @@ run_lift_quant(Exec& ex, bool forward, const pccb200_qpset& qs, const int32_t* q
   return PCCB200_OK;
 }
 
-// predictor order <-> point order helpers of the attribute-level calls
-struct GatherAttrShiftFn {   // out[i] = in[indexes[i]] << 8
+// predictor order <-> point order helpers of the attribute-level calls.  The
+// coefficient rows (stride components per point) may hold several attributes:
+// one attribute's A components start at column off.
+struct GatherAttrShiftFn {   // out[i][off + k] = in[indexes[i]][k] << 8
   const int32_t* in;
   const uint32_t* indexes;
   int A;
+  int stride, off;
   int64_t* out;
   PCC_HD void operator()(int64_t i) const
   {
     for (int k = 0; k < A; k++)
-      out[i * A + k] = int64_t(in[size_t(indexes[i]) * A + k]) << 8;
+      out[i * stride + off + k] = int64_t(in[size_t(indexes[i]) * A + k]) << 8;
   }
 };
 struct GatherQpoFn {
@@ -374,16 +384,17 @@ struct GatherQpoFn {
     out[2 * i + 1] = in[2 * size_t(indexes[i]) + 1];
   }
 };
-struct ScatterReconFn {  // out[indexes[i]] = clip(divExp2RoundHalfInf(in[i], 8))
+struct ScatterReconFn {  // out[indexes[i]][k] = clip(divExp2RoundHalfInf(in[i][off + k], 8))
   const int64_t* in;
   const uint32_t* indexes;
   int A;
+  int stride, off;
   int32_t clipMax;
   int32_t* out;
   PCC_HD void operator()(int64_t i) const
   {
     for (int k = 0; k < A; k++) {
-      int64_t v = div_exp2_round_half_inf(in[i * A + k], 8);
+      int64_t v = div_exp2_round_half_inf(in[i * stride + off + k], 8);
       v = v < 0 ? 0 : (v > clipMax ? clipMax : v);
       out[size_t(indexes[i]) * A + k] = int32_t(v);
     }
@@ -456,6 +467,11 @@ run_quant_weights_scalable(Exec& ex, const uint32_t* numPointsInLod, int lodCoun
   return prevEnd == n ? PCCB200_OK : PCCB200_ERR_INVALID_ARG;
 }
 
+// attr: n rows of A coefficients, predictor order.  Every component goes
+// through the same arithmetic, and the update weights depend on the predictors
+// and the quantisation weights only, so a row may hold several attributes side
+// by side (A = their total component count): each attribute comes out
+// bit-identical to a pass of its own, for the launches of one pass.
 template<class Exec>
 int
 run_lift(Exec& ex, bool forward, const pccb200_predictor* preds, const uint64_t* qw,

@@ -10,7 +10,8 @@
 // (RahtUnit) and share one pipeline: code_raht chooses fused or per-attribute
 // passes and deals the units to lanes, code_units codes a gang of them on one
 // lane.  The attribute-lifting entries (single, slices, a level-of-detail
-// handle; host or device pointers) share code_lift, one LiftUnit per lane.
+// handle, several attribute sets, batches; host or device pointers) share
+// code_lift, one LiftUnit per lane.
 // The recolouring entries (one or several attribute sets, one unit or a batch;
 // host or device pointers) share code_recolour, one RecolourUnit per lane.
 #include <cuda_runtime.h>
@@ -664,74 +665,84 @@ attr_raht_batch(bool forward, bool dev, const pccb200_raht_params* params, int n
 }
 
 // One coding unit of an attribute-lifting call (a slice, or a whole frame): n
-// points, optional point qp offsets ([n, 2]), attributes ([n, A], in and out),
-// values ([n, A], coding order), its row of LCP coefficients (or null).  dev:
-// device pointers, attrs coded in place.  Levels of detail: lod's, or handle's.
+// points, optional point qp offsets ([n, 2]), its levels of detail (lod's, or
+// the handle's) and 1..kLiftMaxSets attribute sets.  Per set: attrsIn ==
+// attrsOut ([n, A], in and out), values ([n, A], coding order) and lcp, the
+// caller's row of PCCB200_MAX_LODS LCP coefficients (or null).  dev: device
+// pointers, attrs coded in place; otherwise host pointers.
 struct LiftUnit {
   int n = 0;
   const int32_t* xyz = nullptr;
   const int32_t* qpo = nullptr;
-  int32_t* attrs = nullptr;
-  int32_t* values = nullptr;
-  int8_t* lcp = nullptr;
   bool dev = false;
   const pccb200_lod_params* lod = nullptr;
   pccb200_lod_handle handle = nullptr;
+  int numSets = 0;
+  LiftSet sets[kLiftMaxSets] = {};
 };
 
-// Validated units, one lane each: stage in, build the levels of detail (or take
-// the handle's), attr_lift_on_lods, stage out.
+// Validated units over at most kCallLanes lanes, one lane each: stage in, build
+// the levels of detail (or take the handle's), attr_lift_on_lods, stage out.
+// nameUnits: a failure's message names the unit.
 int
-code_lift(bool forward, const pccb200_qpset& qpset, bool lcpEnabled, int A, int bitdepth,
-          const std::vector<LiftUnit>& units)
+code_lift(bool forward, const std::vector<LiftUnit>& units, bool nameUnits)
 {
   return parallel_for(int(units.size()), kCallLanes, [&](int i) -> int {
     const LiftUnit& u = units[i];
+    const std::string unit = nameUnits ? "unit " + std::to_string(i) + ": " : std::string();
     pccb200_lod_handle h = u.handle;
     if (h && h->device != ctx().device)
-      return fail(PCCB200_ERR_INVALID_ARG, "handle belongs to another device");
-    const size_t len = size_t(u.n) * A;
+      return fail(PCCB200_ERR_INVALID_ARG, unit + "handle belongs to another device");
     const int levels = u.lod->num_detail_levels;
-    int8_t lcpLocal[PCCB200_MAX_LODS + 1] = {};
-    if (!forward && lcpEnabled && A == 3)
-      for (int l = 0; l < levels && l < PCCB200_MAX_LODS; l++)
-        lcpLocal[l] = u.lcp[l];
+    int8_t lcpLocal[kLiftMaxSets][PCCB200_MAX_LODS + 1] = {};
+    for (int s = 0; s < u.numSets; s++)
+      if (!forward && u.sets[s].lcpEnabled && u.sets[s].A == 3)
+        for (int l = 0; l < levels && l < PCCB200_MAX_LODS; l++)
+          lcpLocal[s][l] = u.sets[s].lcp[l];
     int rc = with_device([&](DeviceExec& ex) -> int {
       const int32_t* dXyz = u.dev || !u.xyz ? u.xyz : to_device(ex, u.xyz, size_t(u.n) * 3);
-      const int32_t* dIn = !forward ? nullptr : u.dev ? u.attrs : to_device(ex, u.attrs, len);
       const int32_t* dQpo = u.dev || !u.qpo ? u.qpo : to_device(ex, u.qpo, size_t(u.n) * 2);
-      int32_t* dV = u.dev     ? u.values
-                    : forward ? ex.alloc<int32_t>(len) : to_device(ex, u.values, len);
-      // (in place: the gather reads attrs before the final write-back overwrites it)
-      int32_t* dOut = u.dev ? u.attrs : ex.alloc<int32_t>(len);
+      LiftSet sets[kLiftMaxSets];
+      for (int s = 0; s < u.numSets; s++) {
+        const LiftSet& t = u.sets[s];
+        const size_t len = size_t(u.n) * t.A;
+        sets[s] = t;
+        sets[s].lcp = lcpLocal[s];
+        if (u.dev)
+          continue;
+        sets[s].attrsIn = forward ? to_device(ex, t.attrsIn, len) : nullptr;
+        sets[s].values = forward ? ex.alloc<int32_t>(len) : to_device(ex, t.values, len);
+        // (in place: the gather reads attrs before the final write-back overwrites it)
+        sets[s].attrsOut = ex.alloc<int32_t>(len);
+      }
       if (h) {
         std::lock_guard<std::mutex> g(h->qwMu);
         if (!h->qwReady) {
           int rcq = run_quant_weights(ex, h->st.preds, u.n, h->st.npl, h->st.lodCount, h->st.qw);
           if (rcq != PCCB200_OK)
-            return fail(rcq, "invalid levels of detail");
+            return fail(rcq, unit + "invalid levels of detail");
           PCC_CUDA_CHECK(cudaStreamSynchronize(ex.stream));  // other lanes read them from now on
           h->qwReady = true;
         }
       }
-      int rc2 = h ? attr_lift_on_lods(ex, forward, h->st, qpset, lcpEnabled, dQpo, dIn, dOut, A,
-                                      bitdepth, dV, lcpLocal)
-                  : attr_lift_run(ex, forward, *u.lod, qpset, lcpEnabled, dQpo, dXyz, dIn, dOut,
-                                  A, u.n, bitdepth, dV, lcpLocal);
+      int rc2 = h ? attr_lift_on_lods(ex, forward, h->st, dQpo, u.numSets, sets)
+                  : attr_lift_run(ex, forward, *u.lod, dQpo, dXyz, u.n, u.numSets, sets);
       if (rc2 != PCCB200_OK)
-        return fail(rc2, rc2 == PCCB200_ERR_UNSUPPORTED
-                           ? "a predictor references its own level of detail"
-                           : "invalid lifting parameters");
-      if (!u.dev) {
-        to_host(ex, u.attrs, dOut, len);
+        return fail(rc2, unit + (rc2 == PCCB200_ERR_UNSUPPORTED
+                                   ? "a predictor references its own level of detail"
+                                   : "invalid lifting parameters"));
+      for (int s = 0; s < u.numSets && !u.dev; s++) {
+        const size_t len = size_t(u.n) * u.sets[s].A;
+        to_host(ex, u.sets[s].attrsOut, sets[s].attrsOut, len);
         if (forward)
-          to_host(ex, u.values, dV, len);
+          to_host(ex, u.sets[s].values, sets[s].values, len);
       }
       return PCCB200_OK;
     });
-    if (rc == PCCB200_OK && forward && u.lcp)
-      for (int l = 0; l < levels && l < PCCB200_MAX_LODS; l++)
-        u.lcp[l] = lcpLocal[l];
+    for (int s = 0; s < u.numSets && rc == PCCB200_OK && forward; s++)
+      if (u.sets[s].lcp)
+        for (int l = 0; l < levels && l < PCCB200_MAX_LODS; l++)
+          u.sets[s].lcp[l] = lcpLocal[s][l];
     return rc;
   });
 }
@@ -766,14 +777,74 @@ attr_lift(bool forward, bool dev, const pccb200_lod_params* lod, pccb200_lod_han
     u.n = int(offs[s + 1] - o);
     u.xyz = h ? nullptr : xyz + 3 * o;
     u.qpo = qpo ? qpo + 2 * o : nullptr;
-    u.attrs = attrs + o * A;
-    u.values = values + o * A;
-    u.lcp = lcp ? lcp + size_t(s) * PCCB200_MAX_LODS : nullptr;
     u.dev = dev;
     u.lod = lod;
     u.handle = h;
+    u.numSets = 1;
+    u.sets[0] = LiftSet{A, bitdepth, qpset, lcpEnabled != 0, attrs + o * A, attrs + o * A,
+                        values + o * A, lcp ? lcp + size_t(s) * PCCB200_MAX_LODS : nullptr};
   }
-  return code_lift(forward, *qpset, lcpEnabled != 0, A, bitdepth, units);
+  return code_lift(forward, units, false);
+}
+
+// Checks the arguments of a pccb200_attr_lift_*_multi* call, before any device
+// is looked up, and describes its units.  Unit u: lods[u], xyz[u], n[u], and
+// per set s attrs / values / lcp[u * numSets + s]; qpsets, lcpEnabled, A and
+// bitdepth are per set.  lcp (the whole array) may be null when no set needs it.
+int
+lift_units(bool forward, bool dev, int numUnits, const pccb200_lod_params* const* lods,
+           int numSets, const pccb200_qpset* const* qpsets, const int32_t* lcpEnabled,
+           const int32_t* const* xyz, const int32_t* n, int32_t* const* attrs, const int32_t* A,
+           const int32_t* bitdepth, int32_t* const* values, int8_t* const* lcp,
+           std::vector<LiftUnit>& units)
+{
+  if (!lods || !qpsets || !lcpEnabled || !xyz || !n || !attrs || !A || !bitdepth || !values
+      || numUnits <= 0 || numSets < 1 || numSets > kLiftMaxSets)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  for (int s = 0; s < numSets; s++)
+    if (!qpsets[s] || (A[s] != 1 && A[s] != 3) || bitdepth[s] < 1 || bitdepth[s] > 16)
+      return fail(PCCB200_ERR_INVALID_ARG,
+                  "set " + std::to_string(s) + ": null qpset, bad component count or bit depth");
+  units.resize(numUnits);
+  for (int i = 0; i < numUnits; i++) {
+    const std::string unit = "unit " + std::to_string(i) + ": ";
+    LiftUnit& u = units[i];
+    u.n = n[i];
+    u.xyz = xyz[i];
+    u.dev = dev;
+    u.lod = lods[i];
+    u.numSets = numSets;
+    if (!u.lod || !u.xyz)
+      return fail(PCCB200_ERR_INVALID_ARG, unit + "null pointer");
+    if (u.n <= 0)
+      return fail(PCCB200_ERR_INVALID_ARG, unit + "no points");
+    for (int s = 0; s < numSets; s++) {
+      const size_t at = size_t(i) * numSets + s;
+      int8_t* row = lcp ? lcp[at] : nullptr;
+      if (!attrs[at] || !values[at])
+        return fail(PCCB200_ERR_INVALID_ARG, unit + "null pointer");
+      if (!forward && lcpEnabled[s] && A[s] == 3 && !row)
+        return fail(PCCB200_ERR_INVALID_ARG, unit + "lcp coefficients missing");
+      u.sets[s] = LiftSet{A[s], bitdepth[s], qpsets[s], lcpEnabled[s] != 0, attrs[at], attrs[at],
+                          values[at], row};
+    }
+  }
+  return PCCB200_OK;
+}
+
+int
+attr_lift_multi(bool forward, bool dev, int numUnits, const pccb200_lod_params* const* lods,
+                int numSets, const pccb200_qpset* const* qpsets, const int32_t* lcpEnabled,
+                const int32_t* const* xyz, const int32_t* n, int32_t* const* attrs,
+                const int32_t* A, const int32_t* bitdepth, int32_t* const* values,
+                int8_t* const* lcp)
+{
+  std::vector<LiftUnit> units;
+  int rc = lift_units(forward, dev, numUnits, lods, numSets, qpsets, lcpEnabled, xyz, n, attrs, A,
+                      bitdepth, values, lcp, units);
+  if (rc != PCCB200_OK)
+    return rc;
+  return code_lift(forward, units, true);
 }
 
 // One unit of a recolouring call (a slice, or a whole frame): source and
@@ -1333,7 +1404,7 @@ lift_quant_common(bool forward, const pccb200_qpset* qpset, const int32_t* qpo,
     int64_t* dA = forward ? to_device(ex, attrs, size_t(n) * A) : ex.alloc<int64_t>(size_t(n) * A);
     int32_t* dV = forward ? ex.alloc<int32_t>(size_t(n) * A) : to_device(ex, values, size_t(n) * A);
     int rc = run_lift_quant(ex, forward, *qpset, dQpo, dQw, n, npl, lodCount, numDetailLevels, dA,
-                            A, lcpEnabled != 0, lcp, dV);
+                            A, 0, A, lcpEnabled != 0, lcp, dV);
     if (rc != PCCB200_OK)
       return fail(rc, "invalid lifting quantisation parameters");
     to_host(ex, attrs, dA, size_t(n) * A);
@@ -1555,6 +1626,108 @@ pccb200_attr_lift_decode_slices_dev(const pccb200_lod_params* lod, const pccb200
   return attr_lift(false, true, lod, nullptr, qpset, lcp_enabled, d_point_qp_offsets, d_xyz,
                    d_attrs_out, num_attrs, bitdepth, slice_offsets, num_slices,
                    const_cast<int32_t*>(d_values_in), const_cast<int8_t*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_multi(const pccb200_lod_params* lod, int32_t num_sets,
+                               const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                               const int32_t* xyz, int32_t n, int32_t* const* attrs_inout,
+                               const int32_t* num_attrs, const int32_t* bitdepths,
+                               int32_t* const* values_out, int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_multi(true, false, 1, &lod, num_sets, qpsets, lcp_enabled, &xyz, &n,
+                         attrs_inout, num_attrs, bitdepths, values_out, lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_multi(const pccb200_lod_params* lod, int32_t num_sets,
+                               const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                               const int32_t* xyz, int32_t n, int32_t* const* attrs_out,
+                               const int32_t* num_attrs, const int32_t* bitdepths,
+                               const int32_t* const* values_in, const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_multi(false, false, 1, &lod, num_sets, qpsets, lcp_enabled, &xyz, &n,
+                         attrs_out, num_attrs, bitdepths, const_cast<int32_t* const*>(values_in),
+                         const_cast<int8_t* const*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_multi_dev(const pccb200_lod_params* lod, int32_t num_sets,
+                                   const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                   const int32_t* d_xyz, int32_t n, int32_t* const* d_attrs_inout,
+                                   const int32_t* num_attrs, const int32_t* bitdepths,
+                                   int32_t* const* d_values_out, int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_multi(true, true, 1, &lod, num_sets, qpsets, lcp_enabled, &d_xyz, &n,
+                         d_attrs_inout, num_attrs, bitdepths, d_values_out, lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_multi_dev(const pccb200_lod_params* lod, int32_t num_sets,
+                                   const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                   const int32_t* d_xyz, int32_t n, int32_t* const* d_attrs_out,
+                                   const int32_t* num_attrs, const int32_t* bitdepths,
+                                   const int32_t* const* d_values_in,
+                                   const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_multi(false, true, 1, &lod, num_sets, qpsets, lcp_enabled, &d_xyz, &n,
+                         d_attrs_out, num_attrs, bitdepths,
+                         const_cast<int32_t* const*>(d_values_in),
+                         const_cast<int8_t* const*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_multi_batch(int32_t num_units, const pccb200_lod_params* const* lods,
+                                     int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                     const int32_t* lcp_enabled, const int32_t* const* xyz,
+                                     const int32_t* n, int32_t* const* attrs_inout,
+                                     const int32_t* num_attrs, const int32_t* bitdepths,
+                                     int32_t* const* values_out, int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_multi(true, false, num_units, lods, num_sets, qpsets, lcp_enabled, xyz, n,
+                         attrs_inout, num_attrs, bitdepths, values_out, lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_multi_batch(int32_t num_units, const pccb200_lod_params* const* lods,
+                                     int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                     const int32_t* lcp_enabled, const int32_t* const* xyz,
+                                     const int32_t* n, int32_t* const* attrs_out,
+                                     const int32_t* num_attrs, const int32_t* bitdepths,
+                                     const int32_t* const* values_in,
+                                     const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_multi(false, false, num_units, lods, num_sets, qpsets, lcp_enabled, xyz, n,
+                         attrs_out, num_attrs, bitdepths, const_cast<int32_t* const*>(values_in),
+                         const_cast<int8_t* const*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_multi_batch_dev(int32_t num_units, const pccb200_lod_params* const* lods,
+                                         int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                         const int32_t* lcp_enabled, const int32_t* const* d_xyz,
+                                         const int32_t* n, int32_t* const* d_attrs_inout,
+                                         const int32_t* num_attrs, const int32_t* bitdepths,
+                                         int32_t* const* d_values_out,
+                                         int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_multi(true, true, num_units, lods, num_sets, qpsets, lcp_enabled, d_xyz, n,
+                         d_attrs_inout, num_attrs, bitdepths, d_values_out, lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_multi_batch_dev(int32_t num_units, const pccb200_lod_params* const* lods,
+                                         int32_t num_sets, const pccb200_qpset* const* qpsets,
+                                         const int32_t* lcp_enabled, const int32_t* const* d_xyz,
+                                         const int32_t* n, int32_t* const* d_attrs_out,
+                                         const int32_t* num_attrs, const int32_t* bitdepths,
+                                         const int32_t* const* d_values_in,
+                                         const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_multi(false, true, num_units, lods, num_sets, qpsets, lcp_enabled, d_xyz, n,
+                         d_attrs_out, num_attrs, bitdepths,
+                         const_cast<int32_t* const*>(d_values_in),
+                         const_cast<int8_t* const*>(lcp_coeffs));
 }
 
 //----------------------------------------------------------------------------

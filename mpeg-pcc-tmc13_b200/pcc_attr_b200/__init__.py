@@ -55,6 +55,7 @@ class Predictor(C.Structure):
 
 
 MAX_LODS = 32
+MAX_LIFT_SETS = 4
 
 
 class LodParams(C.Structure):
@@ -79,8 +80,12 @@ PREDICTOR_DTYPE = np.dtype([("neighbor_count", "<u4"), ("predictor_index", "<u4"
 
 EXPORTS = [
     "pccb200_abi_version", "pccb200_attr_lift_decode", "pccb200_attr_lift_decode_lod",
+    "pccb200_attr_lift_decode_multi", "pccb200_attr_lift_decode_multi_batch",
+    "pccb200_attr_lift_decode_multi_batch_dev", "pccb200_attr_lift_decode_multi_dev",
     "pccb200_attr_lift_decode_slices", "pccb200_attr_lift_decode_slices_dev",
     "pccb200_attr_lift_encode", "pccb200_attr_lift_encode_lod",
+    "pccb200_attr_lift_encode_multi", "pccb200_attr_lift_encode_multi_batch",
+    "pccb200_attr_lift_encode_multi_batch_dev", "pccb200_attr_lift_encode_multi_dev",
     "pccb200_attr_lift_encode_slices", "pccb200_attr_lift_encode_slices_dev",
     "pccb200_attr_raht_decode",
     "pccb200_attr_raht_decode_multi", "pccb200_attr_raht_decode_multi_batch",
@@ -600,6 +605,125 @@ def attr_lift_decode(lod_params, qpset, xyz, values, lcp=None, bitdepth=8, qpoff
         _p(qpoffs, C.c_int32), _p(xyz, C.c_int32), _p(attrs, C.c_int32), C.c_int32(a), C.c_int32(n),
         C.c_int32(bitdepth), _p(values, C.c_int32), _p(l2, C.c_int8)))
     return attrs
+
+
+def _lift_multi_args(lods, qpsets, lcp_enabled, xyzs, attrs, values, lcps, bitdepths, ptr):
+    """C arguments of a pccb200_attr_lift_*_multi_batch(_dev) call: attrs[u][s],
+    values[u][s] (anything ptr() maps to an address), lcps[u][s] host int8 rows
+    of MAX_LODS entries or None"""
+    m, k = len(xyzs), len(qpsets)
+    VP = C.c_void_p * (m * k)
+    return (C.c_int32(m), (C.POINTER(LodParams) * m)(*[C.pointer(lp) for lp in lods]), C.c_int32(k),
+            (C.POINTER(QpSet) * k)(*[C.pointer(q) for q in qpsets]),
+            (C.c_int32 * k)(*[int(e) for e in (lcp_enabled or [0] * k)]),
+            (C.c_void_p * m)(*[ptr(x) for x in xyzs]),
+            (C.c_int32 * m)(*[int(x.shape[0]) for x in xyzs]),
+            VP(*[ptr(a) for u in attrs for a in u]),
+            (C.c_int32 * k)(*[int(a.shape[1]) for a in attrs[0]]),
+            (C.c_int32 * k)(*(bitdepths or [8] * k)),
+            VP(*[ptr(v) for u in values for v in u]),
+            VP(*[None if r is None else r.ctypes.data for u in lcps for r in u]))
+
+
+def attr_lift_multi_batch(forward, lods, qpsets, xyzs, data, lcp_enabled=None, bitdepths=None,
+                          lcps=None):
+    """Several attribute sets of many units (slices / frames) in one lifting call
+    (pccb200_attr_lift_{en,de}code_multi_batch).  lods[u]: LodParams of unit u,
+    xyzs[u]: [N_u, 3]; qpsets, lcp_enabled, bitdepths: per set.
+    forward: data[u][s] = attributes [N_u, A_s] -> (values[u][s] coding order,
+    reconstruction[u][s], lcp[u][s] (num_detail_levels of lods[u] entries)).
+    Otherwise: data[u][s] = values, lcps[u][s] the encoder's lcp rows (or None)
+    -> reconstruction[u][s]."""
+    xyzs = [np.ascontiguousarray(x, dtype=np.int32) for x in xyzs]
+    data = [[np.ascontiguousarray(a, dtype=np.int32).reshape(x.shape[0], -1) for a in u]
+            for x, u in zip(xyzs, data)]
+    if forward:
+        attrs = [[a.copy() for a in u] for u in data]
+        values = [[np.zeros_like(a) for a in u] for u in data]
+        rows = [[np.zeros(MAX_LODS, dtype=np.int8) for _ in u] for u in data]
+    else:
+        attrs = [[np.zeros_like(a) for a in u] for u in data]
+        values = data
+        # a row that is not given stays null, so the library refuses a set that needs it
+        rows = [[None] * len(u) for u in data]
+        for u, lu in zip(rows, lcps if lcps is not None else []):
+            for s, l in enumerate(lu if lu is not None else []):
+                if l is not None:
+                    u[s] = np.zeros(MAX_LODS, dtype=np.int8)
+                    u[s][:len(l)] = l
+    args = _lift_multi_args(lods, qpsets, lcp_enabled, xyzs, attrs, values, rows, bitdepths,
+                            lambda x: x.ctypes.data)
+    fn = (lib().pccb200_attr_lift_encode_multi_batch if forward
+          else lib().pccb200_attr_lift_decode_multi_batch)
+    _check(fn(*args))
+    if not forward:
+        return attrs
+    return values, attrs, [[r[:lp.num_detail_levels].copy() for r in u] for lp, u in zip(lods, rows)]
+
+
+def attr_lift_multi_encode(lod_params, qpsets, xyz, attrs, lcp_enabled=None, bitdepths=None):
+    """several attribute sets of one slice in one lifting pass
+    (pccb200_attr_lift_encode_multi): attrs[s] [N, A_s] -> (values[s] coding
+    order, reconstruction[s], lcp[s] (num_detail_levels entries))"""
+    xyz = np.ascontiguousarray(xyz, dtype=np.int32)
+    attrs = [np.ascontiguousarray(a, dtype=np.int32).reshape(xyz.shape[0], -1).copy() for a in attrs]
+    k = len(attrs)
+    values = [np.zeros_like(a) for a in attrs]
+    rows = [np.zeros(MAX_LODS, dtype=np.int8) for _ in attrs]
+    IP = C.POINTER(C.c_int32) * k
+    _check(lib().pccb200_attr_lift_encode_multi(
+        C.byref(lod_params), C.c_int32(k), (C.POINTER(QpSet) * k)(*[C.pointer(q) for q in qpsets]),
+        (C.c_int32 * k)(*[int(e) for e in (lcp_enabled or [0] * k)]), _p(xyz, C.c_int32),
+        C.c_int32(xyz.shape[0]), IP(*[_p(a, C.c_int32) for a in attrs]),
+        (C.c_int32 * k)(*[a.shape[1] for a in attrs]), (C.c_int32 * k)(*(bitdepths or [8] * k)),
+        IP(*[_p(v, C.c_int32) for v in values]),
+        (C.POINTER(C.c_int8) * k)(*[_p(r, C.c_int8) for r in rows])))
+    return values, attrs, [r[:lod_params.num_detail_levels].copy() for r in rows]
+
+
+def attr_lift_multi_decode(lod_params, qpsets, xyz, values, lcps=None, lcp_enabled=None,
+                           bitdepths=None):
+    """decoder counterpart of attr_lift_multi_encode: values[s] [N, A_s] (coding
+    order), lcps[s] the encoder's lcp coefficients or None -> reconstruction[s]"""
+    xyz = np.ascontiguousarray(xyz, dtype=np.int32)
+    values = [np.ascontiguousarray(v, dtype=np.int32).reshape(xyz.shape[0], -1) for v in values]
+    k = len(values)
+    attrs = [np.zeros_like(v) for v in values]
+    rows = [None] * k
+    for s, l in enumerate(lcps or [None] * k):
+        if l is not None:
+            rows[s] = np.zeros(MAX_LODS, dtype=np.int8)
+            rows[s][:len(l)] = l
+    IP = C.POINTER(C.c_int32) * k
+    _check(lib().pccb200_attr_lift_decode_multi(
+        C.byref(lod_params), C.c_int32(k), (C.POINTER(QpSet) * k)(*[C.pointer(q) for q in qpsets]),
+        (C.c_int32 * k)(*[int(e) for e in (lcp_enabled or [0] * k)]), _p(xyz, C.c_int32),
+        C.c_int32(xyz.shape[0]), IP(*[_p(a, C.c_int32) for a in attrs]),
+        (C.c_int32 * k)(*[v.shape[1] for v in values]), (C.c_int32 * k)(*(bitdepths or [8] * k)),
+        IP(*[_p(v, C.c_int32) for v in values]),
+        (C.POINTER(C.c_int8) * k)(*[_p(r, C.c_int8) for r in rows])))
+    return attrs
+
+
+def attr_lift_multi_batch_dev(forward, lods, qpsets, xyzs, attrs, values, lcps, lcp_enabled=None,
+                              bitdepths=None):
+    """as attr_lift_multi_batch with contiguous int32 torch CUDA tensors (device
+    pointers): xyzs[u], attrs[u][s] (in and out when forward, out otherwise),
+    values[u][s] (out when forward, in otherwise); lcps: host int8 numpy array
+    [units, sets, MAX_LODS] (out when forward, in otherwise).  The producing
+    stream must be synchronised before the call (see the header)."""
+    tensors = list(xyzs) + [a for u in attrs for a in u] + [v for u in values for v in u]
+    for t in tensors:
+        if not (t.is_cuda and t.is_contiguous() and str(t.dtype) == "torch.int32"):
+            raise PccB200Error("attr_lift_multi_batch_dev takes contiguous int32 CUDA tensors")
+    if not (isinstance(lcps, np.ndarray) and lcps.dtype == np.int8 and lcps.flags.c_contiguous
+            and lcps.shape == (len(xyzs), len(qpsets), MAX_LODS)):
+        raise PccB200Error("lcps must be a contiguous int8 array [units, sets, MAX_LODS]")
+    args = _lift_multi_args(lods, qpsets, lcp_enabled, xyzs, attrs, values,
+                            [list(u) for u in lcps], bitdepths, lambda x: x.data_ptr())
+    fn = (lib().pccb200_attr_lift_encode_multi_batch_dev if forward
+          else lib().pccb200_attr_lift_decode_multi_batch_dev)
+    _check(fn(*args))
 
 
 def _i3(v):
