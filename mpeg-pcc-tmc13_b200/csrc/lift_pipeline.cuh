@@ -27,16 +27,20 @@ struct LodState {
   int lodCount;
 };
 
-// fills st (preds / idx / qw must point to n entries each)
+// fills st (preds / idx / qw must point to n entries each).  scal: scalable
+// lifting, whose quantisation weights the encoder computes with (n, 0)
+// (tmc3/AttributeEncoder.cpp:1390-1395) and the decoder with
+// (geom_num_points, min_geom_node_size_log2) (tmc3/AttributeDecoder.cpp:692-697).
 template<class Exec>
 int
 lod_state_build(Exec& ex, const pccb200_lod_params& lod, const int32_t* xyz, int n, LodState& st,
-                bool withWeights = true)
+                bool withWeights = true, const pccb200_lod_scalable* scal = nullptr,
+                bool decoder = false)
 {
   st.n = n;
-  st.numDetailLevels = lod.num_detail_levels;
+  st.numDetailLevels = scal ? kScalableLevels : lod.num_detail_levels;
   st.lodCount = 0;
-  int rc = lod_run(ex, lod, xyz, n, st.preds, st.idx, st.npl, &st.lodCount);
+  int rc = lod_run(ex, lod, xyz, n, st.preds, st.idx, st.npl, &st.lodCount, scal);
   if (rc != PCCB200_OK)
     return rc;
   // (the quantisation weights belong to the lifting transform; a caller that
@@ -44,6 +48,12 @@ lod_state_build(Exec& ex, const pccb200_lod_params& lod, const int32_t* xyz, int
   // stays on the host -- asks for them later)
   if (!withWeights)
     return PCCB200_OK;
+  if (scal) {
+    const bool partial = decoder && scal->geom_num_points;
+    return run_quant_weights_scalable(ex, st.npl, st.lodCount,
+                                      uint64_t(partial ? scal->geom_num_points : n),
+                                      decoder ? scal->min_geom_node_size_log2 : 0, n, st.qw);
+  }
   return run_quant_weights(ex, st.preds, n, st.npl, st.lodCount, st.qw);
 }
 
@@ -133,16 +143,18 @@ attr_lift_on_lods(Exec& ex, bool forward, const LodState& st, const pccb200_qpse
 }
 
 // Levels of detail of xyz [n*3] (executor memory), then attr_lift_on_lods.
+// scal: scalable lifting, or null.
 template<class Exec>
 int
 attr_lift_run(Exec& ex, bool forward, const pccb200_lod_params& lod, const int32_t* qpoIn,
-              const int32_t* xyz, int n, int numSets, const LiftSet* sets)
+              const int32_t* xyz, int n, int numSets, const LiftSet* sets,
+              const pccb200_lod_scalable* scal = nullptr)
 {
   LodState st;
   st.preds = ex.template alloc<pccb200_predictor>(n);
   st.idx = ex.template alloc<uint32_t>(n);
   st.qw = ex.template alloc<uint64_t>(n);
-  int rc = lod_state_build(ex, lod, xyz, n, st);
+  int rc = lod_state_build(ex, lod, xyz, n, st, true, scal, !forward);
   if (rc != PCCB200_OK)
     return rc;
   return attr_lift_on_lods(ex, forward, st, qpoIn, numSets, sets);

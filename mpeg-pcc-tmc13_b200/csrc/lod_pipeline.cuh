@@ -16,6 +16,10 @@
 
 namespace pccb200 {
 
+// levels of detail of scalable lifting: one per octree level
+// (AttributeParameterSet::maxNumDetailLevels, tmc3/hls.h:835-839)
+constexpr int kScalableLevels = 21;
+
 struct FillI32Fn {
   int* p;
   int v;
@@ -47,29 +51,41 @@ build_boxes(Exec& ex, const int32_t* bpos, const uint32_t* list, int count)
 
 // xyz: N x 3 in executor memory.  predsOut / indexesOut: executor memory.
 // nplOut (host, PCCB200_MAX_LODS entries) / lodCountOut (host).
+// scal: scalable lifting (scalable_lifting_enabled_flag), or null.  Then
+// lp.num_detail_levels and lp.dist2 are not read: the levels are the octree
+// levels min_geom_node_size_log2 .. 20 (maxNumDetailLevels(), tmc3/hls.h:835-839).
 template<class Exec>
 int
 lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
-        pccb200_predictor* predsOut, uint32_t* indexesOut, uint32_t* nplOut, int* lodCountOut)
+        pccb200_predictor* predsOut, uint32_t* indexesOut, uint32_t* nplOut, int* lodCountOut,
+        const pccb200_lod_scalable* scal = nullptr)
 {
-  if (N <= 0 || lp.num_detail_levels < 1 || lp.num_detail_levels > PCCB200_MAX_LODS
-      || lp.num_pred_nearest_neighbours < 1 || lp.num_pred_nearest_neighbours > 3
+  if (N <= 0 || lp.num_pred_nearest_neighbours < 1 || lp.num_pred_nearest_neighbours > 3
       || lp.lod_decimation_type < 0 || lp.lod_decimation_type > 2)
     return PCCB200_ERR_INVALID_ARG;
-  // cell shifts are 3 * (dist2 + lod + 1) bits of a 63-bit Morton code
-  if (lp.lod_decimation_type != 1
-      && (lp.dist2 < 0 || lp.dist2 + lp.num_detail_levels > 20))
-    return PCCB200_ERR_INVALID_ARG;
-  if (lp.lod_decimation_type != 0)
-    for (int l = 0; l + 1 < lp.num_detail_levels; l++)
-      if (lp.lod_sampling_period[l] < 2)
-        return PCCB200_ERR_INVALID_ARG;
+  if (scal) {
+    if (lp.lod_decimation_type != 0 || scal->max_neigh_range < 1
+        || scal->min_geom_node_size_log2 < 0 || scal->min_geom_node_size_log2 >= kScalableLevels
+        || (scal->geom_num_points != 0 && scal->geom_num_points < N))
+      return PCCB200_ERR_INVALID_ARG;
+  } else {
+    if (lp.num_detail_levels < 1 || lp.num_detail_levels > PCCB200_MAX_LODS)
+      return PCCB200_ERR_INVALID_ARG;
+    // cell shifts are 3 * (dist2 + lod + 1) bits of a 63-bit Morton code
+    if (lp.lod_decimation_type != 1
+        && (lp.dist2 < 0 || lp.dist2 + lp.num_detail_levels > 20))
+      return PCCB200_ERR_INVALID_ARG;
+    if (lp.lod_decimation_type != 0)
+      for (int l = 0; l + 1 < lp.num_detail_levels; l++)
+        if (lp.lod_sampling_period[l] < 2)
+          return PCCB200_ERR_INVALID_ARG;
+  }
   LodConfig cfg;
-  cfg.numDetailLevels = lp.num_detail_levels;
+  cfg.numDetailLevels = scal ? kScalableLevels : lp.num_detail_levels;
   cfg.decimation = lp.lod_decimation_type;
   for (int i = 0; i < PCCB200_MAX_LODS; i++)
     cfg.samplingPeriod[i] = lp.lod_sampling_period[i];
-  cfg.dist2 = lp.dist2;
+  cfg.dist2 = scal ? 0 : lp.dist2;
   cfg.numNeighbours = lp.num_pred_nearest_neighbours;
   cfg.interRange = lp.inter_lod_search_range;
   cfg.intraRange = lp.intra_lod_search_range;
@@ -78,6 +94,7 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
   for (int k = 0; k < 3; k++)
     cfg.bias[k] = lp.lod_neigh_bias[k];
   cfg.blending = lp.pred_weight_blending != 0;
+  cfg.maxNeighRange = scal ? scal->max_neigh_range : 0;
 
   ex.phase(0);
   int64_t* code = ex.template alloc<int64_t>(N);
@@ -98,7 +115,10 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
 
   uint32_t* input = ex.template alloc<uint32_t>(N);
   uint32_t* retained = ex.template alloc<uint32_t>(N);
-  uint32_t* queries = ex.template alloc<uint32_t>(N);
+  // refined entries of every level in build order (buildPredictorsFast's
+  // indexes before they become point indices): the concatenation of scalable
+  // lifting searches the earlier levels again
+  uint32_t* refined = ex.template alloc<uint32_t>(N);
   uint32_t* indexesBuild = ex.template alloc<uint32_t>(N);
   uint8_t* keep = ex.template alloc<uint8_t>(N);
   int32_t* cellFirst = ex.template alloc<int32_t>(size_t(N) + 1);
@@ -121,9 +141,52 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
   std::vector<uint32_t> npl;
   npl.push_back(uint32_t(N));
   int nInput = N, nIndexes = 0, predBase = N;
+
+  // nearest neighbours of the refined entries queries[0, nQ) of level `lod`
+  // among the retained ones; their predictor slots are predBase - 1 down
+  auto search = [&](int lod, const uint32_t* queries, int nQ, int start, const uint32_t* ret,
+                    int nRet) {
+    ex.phase(2);  // (profiling tag: neighbour search)
+    if (scal)
+      ex.foreach(N, BiasMaskFn{pos, {cfg.bias[0], cfg.bias[1], cfg.bias[2]}, lod, bpos});
+    KnnFn kn;
+    kn.cfg = cfg;
+    kn.v = v;
+    kn.retained = ret;
+    kn.R = nRet;
+    kn.queries = queries;
+    kn.nQueries = nQ;
+    kn.lod = lod;
+    kn.hb = build_boxes(ex, bpos, ret, nRet);
+    if (lod >= cfg.intraSkipLayers)
+      kn.hq = build_boxes(ex, bpos, queries, nQ);
+    else
+      kn.hq = kn.hb;
+    unsigned long long none = ~0ull;
+    ex.upload(dStuck, &none, sizeof(none));
+    const int sb3 = 3 * (1 + cfg.dist2 + lod);
+    ex.foreach(nRet, StuckAtlasFn{code, ret, queries, nQ, sb3 + 21 < 63 ? sb3 + 21 : 63, dStuck});
+    kn.stuck = dStuck;
+    kn.predBase = predBase;
+    kn.indexesOut = indexesBuild + start;
+    kn.p2p = p2p;
+    kn.predCount = predCount;
+    kn.predIdx = predIdx;
+    kn.predW = predW;
+    ex.foreach(nQ, kn);
+    predBase -= nQ;
+  };
+
   const int L = cfg.numDetailLevels;
-  for (int lod = 0; nInput > 0 && lod < L; lod++) {
+  const int lod0 = scal ? scal->min_geom_node_size_log2 : 0;
+  // scalable lifting: layers are concatenated while a level refines more
+  // points than the earlier levels and the skipped points together
+  // (PCCTMC3Common.h:2377-2406)
+  bool concatenate = scal != nullptr;
+  const int64_t skipped = scal && scal->geom_num_points ? scal->geom_num_points - N : 0;
+  for (int lod = lod0; nInput > 0 && lod < L; lod++) {
     const int start = nIndexes;
+    uint32_t* queries = refined + start;
     int nRet = 0, nQ = 0;
     ex.phase(1);  // (profiling tag: subsampling)
     if (lod == L - 1 || nInput == 1 && cfg.decimation != 1) {
@@ -143,7 +206,10 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
       ex.download(&nCells, dCount, sizeof(int));
       int32_t n32 = nInput;
       ex.upload(cellFirst + nCells, &n32, sizeof(int32_t));
-      if (cfg.decimation == 0) {
+      if (scal) {
+        // subsampleByOctree, period 0: every octree node is a segment
+        ex.foreach(nCells, CentroidPickFn{v, input, cellFirst, lod, (lod & 1) != 0, keep});
+      } else if (cfg.decimation == 0) {
         ex.foreach(nCells, FillI32Fn{decision, kCellUndecided});
         SubsampleDistanceFn fn;
         fn.v = v;
@@ -173,7 +239,7 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
         int nSeg = 0;
         ex.download(&nSeg, dCount + 1, sizeof(int));
         ex.upload(segFirst + nSeg, &n32, sizeof(int32_t));
-        ex.foreach(nSeg, CentroidPickFn{v, input, segFirst, cfg.dist2 + lod, keep});
+        ex.foreach(nSeg, CentroidPickFn{v, input, segFirst, cfg.dist2 + lod, true, keep});
       }
       ex.compact(nInput, KeepPred{keep, 1}, ListEmit{input, retained}, dCount + 2);
       ex.compact(nInput, KeepPred{keep, 0}, ListEmit{input, queries}, dCount + 3);
@@ -184,37 +250,23 @@ lod_run(Exec& ex, const pccb200_lod_params& lp, const int32_t* xyz, int N,
     }
     nIndexes += nQ;
 
-    // nearest neighbours of the refined points among the retained ones
-    ex.phase(2);  // (profiling tag: neighbour search)
-    if (nQ > 0) {
-      KnnFn kn;
-      kn.cfg = cfg;
-      kn.v = v;
-      kn.retained = retained;
-      kn.R = nRet;
-      kn.queries = queries;
-      kn.nQueries = nQ;
-      kn.lod = lod;
-      kn.hb = build_boxes(ex, bpos, retained, nRet);
-      if (lod >= cfg.intraSkipLayers)
-        kn.hq = build_boxes(ex, bpos, queries, nQ);
-      else
-        kn.hq = kn.hb;
-      unsigned long long none = ~0ull;
-      ex.upload(dStuck, &none, sizeof(none));
-      const int sb3 = 3 * (1 + cfg.dist2 + lod);
-      ex.foreach(nRet, StuckAtlasFn{code, retained, queries, nQ, sb3 + 21 < 63 ? sb3 + 21 : 63,
-                                    dStuck});
-      kn.stuck = dStuck;
-      kn.predBase = predBase;
-      kn.indexesOut = indexesBuild + start;
-      kn.p2p = p2p;
-      kn.predCount = predCount;
-      kn.predIdx = predIdx;
-      kn.predW = predW;
-      ex.foreach(nQ, kn);
-      predBase -= nQ;
+    if (concatenate && nQ > 0) {
+      if (nQ <= start + skipped) {
+        concatenate = false;
+      } else {
+        // the earlier levels, each at its own lodIndex, against this level's
+        // retained points; their predictor slots are assigned again
+        predBase = N;
+        for (int e = 0; e + 1 < int(npl.size()); e++) {
+          const int s0 = N - int(npl[e]), s1 = N - int(npl[e + 1]);
+          if (s1 > s0)
+            search(lod0 + e, refined + s0, s1 - s0, s0, retained, nRet);
+        }
+      }
     }
+    // nearest neighbours of the refined points among the retained ones
+    if (nQ > 0)
+      search(lod, queries, nQ, start, retained, nRet);
     if (nRet)
       npl.push_back(uint32_t(nRet));
     uint32_t* t = input;

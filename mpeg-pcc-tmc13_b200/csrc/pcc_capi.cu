@@ -676,6 +676,7 @@ struct LiftUnit {
   const int32_t* qpo = nullptr;
   bool dev = false;
   const pccb200_lod_params* lod = nullptr;
+  const pccb200_lod_scalable* scal = nullptr;  // scalable lifting, or null
   pccb200_lod_handle handle = nullptr;
   int numSets = 0;
   LiftSet sets[kLiftMaxSets] = {};
@@ -693,7 +694,7 @@ code_lift(bool forward, const std::vector<LiftUnit>& units, bool nameUnits)
     pccb200_lod_handle h = u.handle;
     if (h && h->device != ctx().device)
       return fail(PCCB200_ERR_INVALID_ARG, unit + "handle belongs to another device");
-    const int levels = u.lod->num_detail_levels;
+    const int levels = u.scal ? kScalableLevels : u.lod->num_detail_levels;
     int8_t lcpLocal[kLiftMaxSets][PCCB200_MAX_LODS + 1] = {};
     for (int s = 0; s < u.numSets; s++)
       if (!forward && u.sets[s].lcpEnabled && u.sets[s].A == 3)
@@ -726,7 +727,7 @@ code_lift(bool forward, const std::vector<LiftUnit>& units, bool nameUnits)
         }
       }
       int rc2 = h ? attr_lift_on_lods(ex, forward, h->st, dQpo, u.numSets, sets)
-                  : attr_lift_run(ex, forward, *u.lod, dQpo, dXyz, u.n, u.numSets, sets);
+                  : attr_lift_run(ex, forward, *u.lod, dQpo, dXyz, u.n, u.numSets, sets, u.scal);
       if (rc2 != PCCB200_OK)
         return fail(rc2, unit + (rc2 == PCCB200_ERR_UNSUPPORTED
                                    ? "a predictor references its own level of detail"
@@ -830,6 +831,51 @@ lift_units(bool forward, bool dev, int numUnits, const pccb200_lod_params* const
     }
   }
   return PCCB200_OK;
+}
+
+// The scalable-lifting arguments a host can check: the encoder codes whole
+// slices (the reference calls AttributeLods::generate with minGeomNodeSizeLog2
+// = 0 and computeQuantizationWeightsScalable with (n, 0)).
+int
+check_scalable(const pccb200_lod_params& lod, const pccb200_lod_scalable& sc, int n, bool encoder,
+               const std::string& unit)
+{
+  if (lod.lod_decimation_type != 0)
+    return fail(PCCB200_ERR_INVALID_ARG, unit + "scalable lifting needs lod_decimation_type 0");
+  if (sc.max_neigh_range < 1 || sc.reserved != 0)
+    return fail(PCCB200_ERR_INVALID_ARG, unit + "max_neigh_range < 1 or reserved not 0");
+  if (sc.min_geom_node_size_log2 < 0 || sc.min_geom_node_size_log2 >= kScalableLevels
+      || (sc.geom_num_points != 0 && sc.geom_num_points < n))
+    return fail(PCCB200_ERR_INVALID_ARG,
+                unit + "min_geom_node_size_log2 out of range or geom_num_points < n");
+  if (encoder && (sc.min_geom_node_size_log2 != 0 || (sc.geom_num_points != 0
+                                                       && sc.geom_num_points != n)))
+    return fail(PCCB200_ERR_INVALID_ARG, unit + "the encoder codes whole slices");
+  return PCCB200_OK;
+}
+
+int
+attr_lift_scalable(bool forward, bool dev, int numUnits, const pccb200_lod_params* const* lods,
+                   const pccb200_lod_scalable* scals, int numSets,
+                   const pccb200_qpset* const* qpsets, const int32_t* lcpEnabled,
+                   const int32_t* const* xyz, const int32_t* n, int32_t* const* attrs,
+                   const int32_t* A, const int32_t* bitdepth, int32_t* const* values,
+                   int8_t* const* lcp)
+{
+  if (!scals)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  std::vector<LiftUnit> units;
+  int rc = lift_units(forward, dev, numUnits, lods, numSets, qpsets, lcpEnabled, xyz, n, attrs, A,
+                      bitdepth, values, lcp, units);
+  if (rc != PCCB200_OK)
+    return rc;
+  for (int i = 0; i < numUnits; i++) {
+    rc = check_scalable(*lods[i], scals[i], n[i], forward, "unit " + std::to_string(i) + ": ");
+    if (rc != PCCB200_OK)
+      return rc;
+    units[i].scal = &scals[i];
+  }
+  return code_lift(forward, units, true);
 }
 
 int
@@ -1328,6 +1374,33 @@ pccb200_lod_build(const pccb200_lod_params* params, const int32_t* xyz, int32_t 
   });
 }
 
+int
+pccb200_lod_build_scalable(const pccb200_lod_params* params, const pccb200_lod_scalable* scal,
+                           const int32_t* xyz, int32_t n, pccb200_predictor* preds_out,
+                           uint32_t* indexes_out, uint32_t* num_points_in_lod_out,
+                           int32_t* lod_count_out)
+{
+  if (!params || !scal || !xyz || !preds_out || !indexes_out || !num_points_in_lod_out
+      || !lod_count_out || n <= 0)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  int rc = check_scalable(*params, *scal, n, false, std::string());
+  if (rc != PCCB200_OK)
+    return rc;
+  return with_device([&](DeviceExec& ex) -> int {
+    int32_t* dXyz = to_device(ex, xyz, size_t(n) * 3);
+    pccb200_predictor* dP = ex.alloc<pccb200_predictor>(n);
+    uint32_t* dIdx = ex.alloc<uint32_t>(n);
+    int cnt = 0;
+    int rc2 = lod_run(ex, *params, dXyz, n, dP, dIdx, num_points_in_lod_out, &cnt, scal);
+    if (rc2 != PCCB200_OK)
+      return fail(rc2, "invalid LoD parameters");
+    *lod_count_out = cnt;
+    to_host(ex, preds_out, dP, size_t(n));
+    to_host(ex, indexes_out, dIdx, size_t(n));
+    return PCCB200_OK;
+  });
+}
+
 // neighWeight: the fixed neighbour weights, or null for the distance-based ones
 static int
 quant_weights_common(const pccb200_predictor* preds, int32_t n, const uint32_t* num_points_in_lod,
@@ -1728,6 +1801,65 @@ pccb200_attr_lift_decode_multi_batch_dev(int32_t num_units, const pccb200_lod_pa
                          d_attrs_out, num_attrs, bitdepths,
                          const_cast<int32_t* const*>(d_values_in),
                          const_cast<int8_t* const*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_scalable(int32_t num_units, const pccb200_lod_params* const* lods,
+                                  const pccb200_lod_scalable* scals, int32_t num_sets,
+                                  const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                  const int32_t* const* xyz, const int32_t* n,
+                                  int32_t* const* attrs_inout, const int32_t* num_attrs,
+                                  const int32_t* bitdepths, int32_t* const* values_out,
+                                  int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_scalable(true, false, num_units, lods, scals, num_sets, qpsets, lcp_enabled,
+                            xyz, n, attrs_inout, num_attrs, bitdepths, values_out,
+                            lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_scalable(int32_t num_units, const pccb200_lod_params* const* lods,
+                                  const pccb200_lod_scalable* scals, int32_t num_sets,
+                                  const pccb200_qpset* const* qpsets, const int32_t* lcp_enabled,
+                                  const int32_t* const* xyz, const int32_t* n,
+                                  int32_t* const* attrs_out, const int32_t* num_attrs,
+                                  const int32_t* bitdepths, const int32_t* const* values_in,
+                                  const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_scalable(false, false, num_units, lods, scals, num_sets, qpsets, lcp_enabled,
+                            xyz, n, attrs_out, num_attrs, bitdepths,
+                            const_cast<int32_t* const*>(values_in),
+                            const_cast<int8_t* const*>(lcp_coeffs));
+}
+
+int
+pccb200_attr_lift_encode_scalable_dev(int32_t num_units, const pccb200_lod_params* const* lods,
+                                      const pccb200_lod_scalable* scals, int32_t num_sets,
+                                      const pccb200_qpset* const* qpsets,
+                                      const int32_t* lcp_enabled, const int32_t* const* d_xyz,
+                                      const int32_t* n, int32_t* const* d_attrs_inout,
+                                      const int32_t* num_attrs, const int32_t* bitdepths,
+                                      int32_t* const* d_values_out, int8_t* const* lcp_coeffs_out)
+{
+  return attr_lift_scalable(true, true, num_units, lods, scals, num_sets, qpsets, lcp_enabled,
+                            d_xyz, n, d_attrs_inout, num_attrs, bitdepths, d_values_out,
+                            lcp_coeffs_out);
+}
+
+int
+pccb200_attr_lift_decode_scalable_dev(int32_t num_units, const pccb200_lod_params* const* lods,
+                                      const pccb200_lod_scalable* scals, int32_t num_sets,
+                                      const pccb200_qpset* const* qpsets,
+                                      const int32_t* lcp_enabled, const int32_t* const* d_xyz,
+                                      const int32_t* n, int32_t* const* d_attrs_out,
+                                      const int32_t* num_attrs, const int32_t* bitdepths,
+                                      const int32_t* const* d_values_in,
+                                      const int8_t* const* lcp_coeffs)
+{
+  return attr_lift_scalable(false, true, num_units, lods, scals, num_sets, qpsets, lcp_enabled,
+                            d_xyz, n, d_attrs_out, num_attrs, bitdepths,
+                            const_cast<int32_t* const*>(d_values_in),
+                            const_cast<int8_t* const*>(lcp_coeffs));
 }
 
 //----------------------------------------------------------------------------

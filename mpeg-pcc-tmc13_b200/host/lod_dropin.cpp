@@ -6,7 +6,7 @@
 //                                        tmc3/AttributeCommon.cpp:45-72)
 //
 // with its exact C++ signature and forwards it to the C ABI of
-// libpcc_attr_b200.so (pccb200_lod_build: Morton sort, subsampling, the
+// libpcc_attr_b200.so (pccb200_lod_build / _scalable: Morton sort, subsampling, the
 // nearest-neighbour search, predictor weights incl. blending).  The callers
 // AttributeEncoder::encode (tmc3/AttributeEncoder.cpp:456-460) and
 // AttributeDecoder::decode (tmc3/AttributeDecoder.cpp:229-233) are unchanged:
@@ -17,8 +17,9 @@
 // It is linked INSTEAD of the reference's definition: oracle/Makefile renames
 // that one symbol in AttributeCommon.o (objcopy --redefine-sym) to
 // pccb200_reference_lods_generate, which this unit keeps for the parameter
-// combinations the library does not cover (scalable lifting, canonical point
-// order, inter-frame references).  A maintainer would instead rename the
+// combinations the library does not cover (canonical point order, inter-frame
+// references).  Scalable lifting, partial decodes included, goes to
+// pccb200_lod_build_scalable.  A maintainer would instead rename the
 // function in AttributeCommon.cpp; see INTEGRATION.md.
 #include <stdexcept>
 #include <string>
@@ -47,10 +48,15 @@ AttributeLods::generate(
   const AttributeInterPredParams& attrInterPredParams)
 {
   const int n = int(cloud.getPointCount());
-  const bool covered = !aps.scalable_lifting_enabled_flag && minGeomNodeSizeLog2 == 0
+  const bool scalable = aps.scalable_lifting_enabled_flag;
+  // scalable lifting, including a partial decode (minGeomNodeSizeLog2 > 0)
+  const bool levelsCovered = scalable
+    ? int(aps.lod_decimation_type) == 0 && minGeomNodeSizeLog2 >= 0 && minGeomNodeSizeLog2 < 21
+      && int64_t(geom_num_points_minus1) + 1 >= n
+    : minGeomNodeSizeLog2 == 0 && aps.num_detail_levels_minus1 + 1 <= PCCB200_MAX_LODS;
+  const bool covered = levelsCovered
     && !aps.canonical_point_order_flag && aps.max_points_per_sort_log2_plus1 == 0
     && !attrInterPredParams.enableAttrInterPred && n > 0
-    && aps.num_detail_levels_minus1 + 1 <= PCCB200_MAX_LODS
     && aps.num_pred_nearest_neighbours_minus1 < 3;
   if (!covered) {
     pccb200_reference_lods_generate(
@@ -87,7 +93,14 @@ AttributeLods::generate(
   indexes.resize(n);
   uint32_t npl[PCCB200_MAX_LODS] = {};
   int32_t lodCount = 0;
-  int rc = pccb200_lod_build(&lp, xyz.data(), n, flat.data(), indexes.data(), npl, &lodCount);
+  pccb200_lod_scalable scal = {};
+  scal.max_neigh_range = aps.max_neigh_range_minus1 + 1;
+  scal.min_geom_node_size_log2 = minGeomNodeSizeLog2;
+  scal.geom_num_points = int64_t(geom_num_points_minus1) + 1;
+  int rc = scalable
+    ? pccb200_lod_build_scalable(&lp, &scal, xyz.data(), n, flat.data(), indexes.data(), npl,
+                                 &lodCount)
+    : pccb200_lod_build(&lp, xyz.data(), n, flat.data(), indexes.data(), npl, &lodCount);
   if (rc != PCCB200_OK)
     throw std::runtime_error(
       std::string("pcc_attr_b200: LoD build failed: ") + pccb200_last_error());

@@ -75,6 +75,20 @@ class LodParams(C.Structure):
     ]
 
 
+class LodScalable(C.Structure):
+    """pccb200_lod_scalable: scalable lifting beside a LodParams.  geom_num_points
+    0 means n (the encoder, and every full decode)."""
+    _fields_ = [
+        ("max_neigh_range", C.c_int32),
+        ("min_geom_node_size_log2", C.c_int32),
+        ("geom_num_points", C.c_int64),
+        ("reserved", C.c_int32),
+    ]
+
+
+# levels of detail of scalable lifting (maxNumDetailLevels)
+SCALABLE_LODS = 21
+
 PREDICTOR_DTYPE = np.dtype([("neighbor_count", "<u4"), ("predictor_index", "<u4", 3),
                             ("weight", "<u4", 3)])
 
@@ -82,10 +96,12 @@ EXPORTS = [
     "pccb200_abi_version", "pccb200_attr_lift_decode", "pccb200_attr_lift_decode_lod",
     "pccb200_attr_lift_decode_multi", "pccb200_attr_lift_decode_multi_batch",
     "pccb200_attr_lift_decode_multi_batch_dev", "pccb200_attr_lift_decode_multi_dev",
+    "pccb200_attr_lift_decode_scalable", "pccb200_attr_lift_decode_scalable_dev",
     "pccb200_attr_lift_decode_slices", "pccb200_attr_lift_decode_slices_dev",
     "pccb200_attr_lift_encode", "pccb200_attr_lift_encode_lod",
     "pccb200_attr_lift_encode_multi", "pccb200_attr_lift_encode_multi_batch",
     "pccb200_attr_lift_encode_multi_batch_dev", "pccb200_attr_lift_encode_multi_dev",
+    "pccb200_attr_lift_encode_scalable", "pccb200_attr_lift_encode_scalable_dev",
     "pccb200_attr_lift_encode_slices", "pccb200_attr_lift_encode_slices_dev",
     "pccb200_attr_raht_decode",
     "pccb200_attr_raht_decode_multi", "pccb200_attr_raht_decode_multi_batch",
@@ -97,7 +113,8 @@ EXPORTS = [
     "pccb200_attr_raht_encode_symbols", "pccb200_attr_spherical_positions",
     "pccb200_coeff_symbols", "pccb200_estimate_dist2", "pccb200_kernel_launch_count",
     "pccb200_last_error", "pccb200_lift_dequantize", "pccb200_lift_forward",
-    "pccb200_lift_inverse", "pccb200_lift_quantize", "pccb200_lod_build", "pccb200_lod_create",
+    "pccb200_lift_inverse", "pccb200_lift_quantize", "pccb200_lod_build",
+    "pccb200_lod_build_scalable", "pccb200_lod_create",
     "pccb200_lod_destroy", "pccb200_lod_info", "pccb200_lod_reusable", "pccb200_morton_sort",
     "pccb200_offset_and_scale", "pccb200_profile_enable", "pccb200_profile_read",
     "pccb200_profile_reset", "pccb200_quant_weights", "pccb200_quant_weights_fixed",
@@ -561,6 +578,22 @@ def lod_build(params, xyz):
     return preds, indexes, npl[:cnt.value].copy()
 
 
+def lod_build_scalable(params, scal, xyz):
+    """scalable lifting (pccb200_lod_build_scalable): params LodParams, scal
+    LodScalable -> (predictors[N], indexes[N], num_points_in_lod[lods])"""
+    xyz = np.ascontiguousarray(xyz, dtype=np.int32)
+    n = xyz.shape[0]
+    preds = np.zeros(n, dtype=PREDICTOR_DTYPE)
+    indexes = np.zeros(n, dtype=np.uint32)
+    npl = np.zeros(MAX_LODS, dtype=np.uint32)
+    cnt = C.c_int32(0)
+    _check(lib().pccb200_lod_build_scalable(
+        C.byref(params), C.byref(scal), _p(xyz, C.c_int32), C.c_int32(n),
+        C.cast(preds.ctypes.data, C.POINTER(Predictor)), _p(indexes, C.c_uint32),
+        _p(npl, C.c_uint32), C.byref(cnt)))
+    return preds, indexes, npl[:cnt.value].copy()
+
+
 def attr_lift_encode(lod_params, qpset, xyz, attrs, lcp_enabled=0, bitdepth=8, qpoffs=None):
     """-> (values [N,A] coding order, reconstruction [N,A] point order, lcp coefficients)"""
     xyz = np.ascontiguousarray(xyz, dtype=np.int32)
@@ -724,6 +757,59 @@ def attr_lift_multi_batch_dev(forward, lods, qpsets, xyzs, attrs, values, lcps, 
     fn = (lib().pccb200_attr_lift_encode_multi_batch_dev if forward
           else lib().pccb200_attr_lift_decode_multi_batch_dev)
     _check(fn(*args))
+
+
+def _scalable_args(scals, args):
+    """a *_multi_batch argument tuple with the LodScalable array after lods"""
+    return args[:2] + ((LodScalable * len(scals))(*scals),) + args[2:]
+
+
+def attr_lift_scalable(forward, lods, scals, qpsets, xyzs, data, lcp_enabled=None,
+                       bitdepths=None, lcps=None):
+    """Scalable lifting (pccb200_attr_lift_{en,de}code_scalable), shaped as
+    attr_lift_multi_batch with scals[u] the LodScalable of unit u.  lcp rows
+    have SCALABLE_LODS entries."""
+    xyzs = [np.ascontiguousarray(x, dtype=np.int32) for x in xyzs]
+    data = [[np.ascontiguousarray(a, dtype=np.int32).reshape(x.shape[0], -1) for a in u]
+            for x, u in zip(xyzs, data)]
+    if forward:
+        attrs = [[a.copy() for a in u] for u in data]
+        values = [[np.zeros_like(a) for a in u] for u in data]
+        rows = [[np.zeros(MAX_LODS, dtype=np.int8) for _ in u] for u in data]
+    else:
+        attrs = [[np.zeros_like(a) for a in u] for u in data]
+        values = data
+        rows = [[None] * len(u) for u in data]
+        for u, lu in zip(rows, lcps if lcps is not None else []):
+            for s, l in enumerate(lu if lu is not None else []):
+                if l is not None:
+                    u[s] = np.zeros(MAX_LODS, dtype=np.int8)
+                    u[s][:len(l)] = l
+    args = _lift_multi_args(lods, qpsets, lcp_enabled, xyzs, attrs, values, rows, bitdepths,
+                            lambda x: x.ctypes.data)
+    fn = (lib().pccb200_attr_lift_encode_scalable if forward
+          else lib().pccb200_attr_lift_decode_scalable)
+    _check(fn(*_scalable_args(scals, args)))
+    if not forward:
+        return attrs
+    return values, attrs, [[r[:SCALABLE_LODS].copy() for r in u] for u in rows]
+
+
+def attr_lift_scalable_dev(forward, lods, scals, qpsets, xyzs, attrs, values, lcps,
+                           lcp_enabled=None, bitdepths=None):
+    """as attr_lift_multi_batch_dev, for scalable lifting (scals[u] per unit)"""
+    tensors = list(xyzs) + [a for u in attrs for a in u] + [v for u in values for v in u]
+    for t in tensors:
+        if not (t.is_cuda and t.is_contiguous() and str(t.dtype) == "torch.int32"):
+            raise PccB200Error("attr_lift_scalable_dev takes contiguous int32 CUDA tensors")
+    if not (isinstance(lcps, np.ndarray) and lcps.dtype == np.int8 and lcps.flags.c_contiguous
+            and lcps.shape == (len(xyzs), len(qpsets), MAX_LODS)):
+        raise PccB200Error("lcps must be a contiguous int8 array [units, sets, MAX_LODS]")
+    args = _lift_multi_args(lods, qpsets, lcp_enabled, xyzs, attrs, values,
+                            [list(u) for u in lcps], bitdepths, lambda x: x.data_ptr())
+    fn = (lib().pccb200_attr_lift_encode_scalable_dev if forward
+          else lib().pccb200_attr_lift_decode_scalable_dev)
+    _check(fn(*_scalable_args(scals, args)))
 
 
 def _i3(v):
