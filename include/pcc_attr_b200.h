@@ -424,6 +424,59 @@ int pccb200_recolour_multi_batch_dev(const pccb200_recolour_params* params, int3
                                      const int32_t* const* d_target_xyz, const int32_t* n_target,
                                      int32_t* const* d_target_attrs_out);
 
+/* Reference-exact recolouring --
+ *
+ * The entries above find their neighbours over a grid hash and break distance
+ * ties by the lower point index.  These find them as the reference encoder
+ * does: they build the kd-tree nanoflann builds for
+ * KDTreeVectorOfVectorsAdaptor<PCCPointSet3, double> (metric_L2, leaf size 10),
+ * on the device, level by level, and run nanoflann's findNeighbors on it, one
+ * thread per query, with the same arithmetic; among equidistant candidates the
+ * one nanoflann's traversal meets first is kept, as in the reference.  Each
+ * target's backward list is put in the order libstdc++'s std::sort (g++ 13)
+ * leaves it, which decides the order of the sums that follow.  The result
+ * equals recolourColour / recolourReflectance (tmc3/pointset_processing.cpp)
+ * bit for bit, ties, duplicate points and non-dyadic scales included.  The
+ * two families differ on purpose wherever a distance tie reaches the k-th
+ * neighbour.
+ *
+ * Same arguments and same rules as pccb200_recolour,
+ * pccb200_recolour_multi_batch and pccb200_recolour_multi_batch_dev, except
+ * the coordinate range: any int32 coordinate and offset of |x| < 2^30 (so that
+ * target + offset cannot overflow); one outside it returns
+ * PCCB200_ERR_INVALID_ARG, found on the device.  The other arguments are
+ * checked before any device lookup.  The position-only work (both trees, both
+ * searches, the backward lists) runs once per unit for all sets.
+ *
+ * Workspace of a unit in flight: up to about 300 bytes per point on either
+ * side for the two trees and their build, on top of the lists of the entries
+ * above. */
+int pccb200_recolour_exact(const pccb200_recolour_params* params, const int32_t* source_xyz,
+                           const int32_t* source_attrs, int32_t num_attrs, int32_t n_source,
+                           double source_to_target_scale, const int32_t tgt_to_src_offset[3],
+                           const int32_t* target_xyz, int32_t n_target, int32_t bitdepth,
+                           int32_t* target_attrs_out);
+int pccb200_recolour_exact_multi_batch(const pccb200_recolour_params* params, int32_t num_sets,
+                                       int32_t num_units,
+                                       const int32_t* const* source_xyz, const int32_t* n_source,
+                                       const int32_t* const* source_attrs,
+                                       const int32_t* num_attrs, const int32_t* bitdepths,
+                                       const double* source_to_target_scale,
+                                       const int32_t* tgt_to_src_offsets,
+                                       const int32_t* const* target_xyz, const int32_t* n_target,
+                                       int32_t* const* target_attrs_out);
+int pccb200_recolour_exact_multi_batch_dev(const pccb200_recolour_params* params,
+                                           int32_t num_sets, int32_t num_units,
+                                           const int32_t* const* d_source_xyz,
+                                           const int32_t* n_source,
+                                           const int32_t* const* d_source_attrs,
+                                           const int32_t* num_attrs, const int32_t* bitdepths,
+                                           const double* source_to_target_scale,
+                                           const int32_t* tgt_to_src_offsets,
+                                           const int32_t* const* d_target_xyz,
+                                           const int32_t* n_target,
+                                           int32_t* const* d_target_attrs_out);
+
 /* Per-phase device timing (CUDA events around every kernel launch on
  * the call's stream).  Phases: 0 Morton keys + radix sort, 1 tree build
  * (histogram, compaction, leaf / merge kernels), 2 block transform (the

@@ -906,6 +906,7 @@ struct RecolourUnit {
   bool dev = false;
   int numSets = 0;
   RecolourSet sets[kRecolourMaxSets] = {};
+  RecolourSearch search = kRecolourGrid;
 };
 
 // Validated units over at most kCallLanes lanes, one lane each: stage in,
@@ -927,11 +928,15 @@ code_recolour(const pccb200_recolour_params& rp, const std::vector<RecolourUnit>
       const int32_t* dTgt = u.dev ? u.tgtXyz : to_device(ex, u.tgtXyz, size_t(u.nTgt) * 3);
       for (int s = 0; s < u.numSets && !u.dev; s++)
         sets[s].out = ex.alloc<int32_t>(size_t(u.nTgt) * u.sets[s].A);
-      int rc = recolour_run(ex, rp, dSrc, u.nSrc, u.scale, u.off, dTgt, u.nTgt, u.numSets, sets);
+      int rc = recolour_run(ex, rp, dSrc, u.nSrc, u.scale, u.off, dTgt, u.nTgt, u.numSets, sets,
+                            u.search);
       if (rc != PCCB200_OK)
         return fail(rc, (nameUnits ? "unit " + std::to_string(i) + ": " : std::string())
-                          + "invalid recolouring parameters (neighbour counts, scale, or a "
-                            "coordinate outside [0, 2^21))");
+                          + (u.search == kRecolourRefExact
+                               ? "invalid recolouring parameters (neighbour counts, scale, or a "
+                                 "coordinate or offset outside (-2^30, 2^30))"
+                               : "invalid recolouring parameters (neighbour counts, scale, or a "
+                                 "coordinate outside [0, 2^21))"));
       for (int s = 0; s < u.numSets && !u.dev; s++)
         to_host(ex, u.sets[s].out, sets[s].out, size_t(u.nTgt) * u.sets[s].A);
       return PCCB200_OK;
@@ -947,7 +952,8 @@ recolour_units(bool dev, const pccb200_recolour_params* params, int numSets, int
                const int32_t* const* srcXyz, const int32_t* nSrc,
                const int32_t* const* srcAttrs, const int32_t* A, const int32_t* bitdepth,
                const double* scale, const int32_t* offsets, const int32_t* const* tgtXyz,
-               const int32_t* nTgt, int32_t* const* out, std::vector<RecolourUnit>& units)
+               const int32_t* nTgt, int32_t* const* out, std::vector<RecolourUnit>& units,
+               RecolourSearch search)
 {
   if (!params || !srcXyz || !nSrc || !srcAttrs || !A || !bitdepth || !scale || !offsets
       || !tgtXyz || !nTgt || !out || numUnits <= 0 || numSets < 1 || numSets > kRecolourMaxSets)
@@ -964,6 +970,7 @@ recolour_units(bool dev, const pccb200_recolour_params* params, int numSets, int
       u.off[k] = offsets[3 * size_t(i) + k];
     u.dev = dev;
     u.numSets = numSets;
+    u.search = search;
     bool null = !u.srcXyz || !u.tgtXyz;
     for (int s = 0; s < numSets; s++) {
       const size_t at = size_t(i) * numSets + s;
@@ -985,11 +992,11 @@ recolour_multi(bool dev, const pccb200_recolour_params* params, int numSets, int
                const int32_t* const* srcXyz, const int32_t* nSrc,
                const int32_t* const* srcAttrs, const int32_t* A, const int32_t* bitdepth,
                const double* scale, const int32_t* offsets, const int32_t* const* tgtXyz,
-               const int32_t* nTgt, int32_t* const* out)
+               const int32_t* nTgt, int32_t* const* out, RecolourSearch search = kRecolourGrid)
 {
   std::vector<RecolourUnit> units;
   int rc = recolour_units(dev, params, numSets, numUnits, srcXyz, nSrc, srcAttrs, A, bitdepth,
-                          scale, offsets, tgtXyz, nTgt, out, units);
+                          scale, offsets, tgtXyz, nTgt, out, units, search);
   if (rc != PCCB200_OK)
     return rc;
   return code_recolour(*params, units, true);
@@ -2162,6 +2169,55 @@ pccb200_recolour_multi_batch_dev(const pccb200_recolour_params* params, int32_t 
   return recolour_multi(true, params, num_sets, num_units, d_source_xyz, n_source, d_source_attrs,
                         num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
                         d_target_xyz, n_target, d_target_attrs_out);
+}
+
+// the reference-exact recolouring: nanoflann's trees and search, std::sort's
+// list order (recolour.cuh, kRecolourRefExact)
+
+int
+pccb200_recolour_exact(const pccb200_recolour_params* params, const int32_t* source_xyz,
+                       const int32_t* source_attrs, int32_t num_attrs, int32_t n_source,
+                       double source_to_target_scale, const int32_t tgt_to_src_offset[3],
+                       const int32_t* target_xyz, int32_t n_target, int32_t bitdepth,
+                       int32_t* target_attrs_out)
+{
+  if (!params || !source_xyz || !source_attrs || !tgt_to_src_offset || !target_xyz
+      || !target_attrs_out)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  return recolour_multi(false, params, 1, 1, &source_xyz, &n_source, &source_attrs, &num_attrs,
+                        &bitdepth, &source_to_target_scale, tgt_to_src_offset, &target_xyz,
+                        &n_target, &target_attrs_out, kRecolourRefExact);
+}
+
+int
+pccb200_recolour_exact_multi_batch(const pccb200_recolour_params* params, int32_t num_sets,
+                                   int32_t num_units, const int32_t* const* source_xyz,
+                                   const int32_t* n_source, const int32_t* const* source_attrs,
+                                   const int32_t* num_attrs, const int32_t* bitdepths,
+                                   const double* source_to_target_scale,
+                                   const int32_t* tgt_to_src_offsets,
+                                   const int32_t* const* target_xyz, const int32_t* n_target,
+                                   int32_t* const* target_attrs_out)
+{
+  return recolour_multi(false, params, num_sets, num_units, source_xyz, n_source, source_attrs,
+                        num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
+                        target_xyz, n_target, target_attrs_out, kRecolourRefExact);
+}
+
+int
+pccb200_recolour_exact_multi_batch_dev(const pccb200_recolour_params* params, int32_t num_sets,
+                                       int32_t num_units, const int32_t* const* d_source_xyz,
+                                       const int32_t* n_source,
+                                       const int32_t* const* d_source_attrs,
+                                       const int32_t* num_attrs, const int32_t* bitdepths,
+                                       const double* source_to_target_scale,
+                                       const int32_t* tgt_to_src_offsets,
+                                       const int32_t* const* d_target_xyz,
+                                       const int32_t* n_target, int32_t* const* d_target_attrs_out)
+{
+  return recolour_multi(true, params, num_sets, num_units, d_source_xyz, n_source, d_source_attrs,
+                        num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
+                        d_target_xyz, n_target, d_target_attrs_out, kRecolourRefExact);
 }
 
 }  // extern "C"

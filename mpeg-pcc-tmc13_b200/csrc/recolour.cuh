@@ -16,11 +16,14 @@
 // index, which nanoflann does not promise -- see DESIGN.md for what that
 // means for parity (bit-exact against the oracle, which restates the same
 // rule; within a stated tolerance of the compiled reference on clouds where
-// distance ties reach the k-th neighbour).
+// distance ties reach the k-th neighbour).  The second path (kRecolourRefExact)
+// searches nanoflann's own tree instead (kdtree.cuh) and orders the backward
+// lists as std::sort does: equal to the reference bit for bit.
 #pragma once
 
 #include <math.h>
 
+#include "kdtree.cuh"    // dmul / dadd / dsub, the reference-exact search
 #include "raht_core.cuh"
 #include "spherical.cuh"  // atomic_min_i32 / atomic_max_i32
 
@@ -54,36 +57,6 @@ struct RecolourSet {
   int32_t* refined1;
   int32_t* out;
 };
-
-// exact products and sums (the compiler must not contract them into FMAs:
-// the reference is built without)
-PCC_HD double
-dmul(double a, double b)
-{
-#if defined(__CUDA_ARCH__)
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-PCC_HD double
-dadd(double a, double b)
-{
-#if defined(__CUDA_ARCH__)
-  return __dadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
-PCC_HD double
-dsub(double a, double b)
-{
-#if defined(__CUDA_ARCH__)
-  return __dsub_rn(a, b);
-#else
-  return a - b;
-#endif
-}
 
 PCC_HD int
 atomic_fetch_add_i32(int* p, int v)
@@ -309,6 +282,34 @@ struct KnnQueryFn {
   }
 };
 
+// the same queries through nanoflann's tree and search (kdtree.cuh)
+struct KdKnnQueryFn {
+  KdTree T;
+  RecolourConfig cfg;
+  const int32_t* qxyz;
+  int backward;
+  int k;
+  double* outDist;    // nQueries x k
+  int32_t* outIdx;
+  PCC_HD void operator()(int64_t i) const
+  {
+    double q[3];
+    for (int c = 0; c < 3; c++) {
+      if (backward)
+        q[c] = dsub(dmul(double(qxyz[3 * i + c]), cfg.scale), double(cfg.off[c]));
+      else
+        q[c] = dmul(double(qxyz[3 * i + c] + cfg.off[c]), cfg.invScale);
+    }
+    KdResult R;
+    R.init(k);
+    kd_find_neighbours(T, q, R);
+    for (int j = 0; j < k; j++) {
+      outDist[size_t(i) * k + j] = j < R.count ? R.d[j] : 0.0;
+      outIdx[size_t(i) * k + j] = j < R.count ? R.id[j] : -1;
+    }
+  }
+};
+
 // The reference pops its result vectors when the k-th neighbour is farther
 // than maxGeometryDist2Fwd -- and never restores them (the vectors live
 // outside the loop, pointset_processing.cpp:301-326): from the first such
@@ -333,8 +334,12 @@ clip_round(double v, double hi)
 }
 
 // forward colour of every target (pointset_processing.cpp:301-399 / :660-744):
-// one thread per target, its neighbour list read once for every set
-struct ForwardColourFn {
+// one thread per target, its neighbour list read once for every set.
+// kRefExact: the attribute distance of a colour is taken as the reference
+// takes it, on Vec3<attr_t> differences (:337-348), each component wrapped to
+// uint16 before it is squared; a reflectance difference is a plain int (:709).
+template<bool kRefExact>
+struct ForwardColourT {
   RecolourConfig cfg;
   const double* dist;     // nTgt x kFwd
   const int32_t* idx;
@@ -362,8 +367,12 @@ struct ForwardColourFn {
           for (int j = 0; j < nNN; j++) {
             double s = 0.0;
             for (int c = 0; c < A; c++) {
-              const double df = double(srcAttr[size_t(id[i]) * A + c])
+              double df = double(srcAttr[size_t(id[i]) * A + c])
                 - double(srcAttr[size_t(id[j]) * A + c]);
+              if constexpr (kRefExact) {
+                if (A == 3)
+                  df = double(uint16_t(srcAttr[size_t(id[i]) * A + c] - srcAttr[size_t(id[j]) * A + c]));
+              }
               s = dadd(s, dmul(df, df));
             }
             if (s > maxAttr)
@@ -401,6 +410,8 @@ struct ForwardColourFn {
     }
   }
 };
+
+using ForwardColourFn = ForwardColourT<false>;
 
 // backward lists: the sources that name a target among their kBwd nearest
 // (pointset_processing.cpp:409-428), as CSR: count, (scan), fill, sort.
@@ -443,11 +454,15 @@ struct BackwardFillFn {
 
 // final colour of every target (pointset_processing.cpp:430-611 / :773-921):
 // one thread per target sorts its backward list once, then runs the centroid
-// and the search of every set
-struct FinalColourFn {
+// and the search of every set.  kRefOrder = false: the list is ordered by
+// (dist, source index).  kRefOrder = true: in the order the reference's
+// std::sort on distance leaves it -- the list as it was pushed (by source
+// index), then libstdc++'s introsort (GnuSort) keyed on distance alone.
+template<bool kRefOrder>
+struct FinalColourT {
   RecolourConfig cfg;
   const int* first;
-  double* listDist;     // sorted in place by (dist, source index)
+  double* listDist;     // sorted in place (see kRefOrder)
   int32_t* listSrc;
   int numSets;
   RecolourSet sets[kRecolourMaxSets];
@@ -463,19 +478,24 @@ struct FinalColourFn {
           sets[si].out[size_t(t) * sets[si].A + c] = sets[si].refined1[size_t(t) * sets[si].A + c];
       return;
     }
-    // std::sort by distance (the reference's order among equal distances is
-    // unspecified; here: by source index)
-    for (int i = 1; i < L0; i++) {
-      const double d = ld[i];
-      const int32_t s = ls[i];
-      int p = i;
-      while (p > 0 && (ld[p - 1] > d || (ld[p - 1] == d && ls[p - 1] > s))) {
-        ld[p] = ld[p - 1];
-        ls[p] = ls[p - 1];
-        p--;
+    if constexpr (kRefOrder) {
+      GnuSort<int32_t, double, IndexLess>{ls, ld, IndexLess{}}(L0);
+      GnuSort<double, int32_t, DistLess>{ld, ls, DistLess{}}(L0);
+    } else {
+      // std::sort by distance (the reference's order among equal distances is
+      // unspecified; here: by source index)
+      for (int i = 1; i < L0; i++) {
+        const double d = ld[i];
+        const int32_t s = ls[i];
+        int p = i;
+        while (p > 0 && (ld[p - 1] > d || (ld[p - 1] == d && ls[p - 1] > s))) {
+          ld[p] = ld[p - 1];
+          ls[p] = ls[p - 1];
+          p--;
+        }
+        ld[p] = d;
+        ls[p] = s;
       }
-      ld[p] = d;
-      ls[p] = s;
     }
     for (int si = 0; si < numSets; si++) {
       const RecolourSet& S = sets[si];
@@ -580,6 +600,8 @@ struct FinalColourFn {
   }
 };
 
+using FinalColourFn = FinalColourT<false>;
+
 struct FillI32ValueFn {
   int32_t* p;
   int32_t v;
@@ -630,7 +652,8 @@ build_point_grid(Exec& ex, const int32_t* xyz, int n, PointGrid& g)
 // The arguments recolour_run accepts: at least one point on each side, 1 to
 // kRecolourMaxSets sets of 1 or 3 components at 1 to 16 bits, neighbour counts
 // within kRecolourMaxK and the point counts, a search range of 0 to 8 and a
-// positive scale.  (Coordinates outside [0, 2^21) are found by build_point_grid.)
+// positive scale.  (Coordinates outside [0, 2^21) are found by build_point_grid,
+// those outside (-2^30, 2^30) of the reference-exact search by kd_coords_valid.)
 inline bool
 recolour_args_valid(const pccb200_recolour_params& rp, int nSrc, int nTgt, double scale,
                     int numSets, const RecolourSet* sets)
@@ -647,20 +670,47 @@ recolour_args_valid(const pccb200_recolour_params& rp, int nSrc, int nTgt, doubl
   return true;
 }
 
+// The neighbour search and backward-list order of a recolour_run call.
+//   kRecolourGrid: exact k nearest over grid hashes, ties by the lower point
+//     index, lists by (dist, source index); coordinates in [0, 2^21).
+//   kRecolourRefExact: nanoflann's trees and traversal (kdtree.cuh), lists in
+//     libstdc++'s std::sort order: the reference's recolourColour /
+//     recolourReflectance bit for bit; coordinates (and offsets) of |x| < 2^30.
+enum RecolourSearch { kRecolourGrid = 0, kRecolourRefExact = 1 };
+
+// |x| < 2^30 for every coordinate of both sides and the offset
+template<class Exec>
+bool
+kd_coords_valid(Exec& ex, const int32_t* srcXyz, int nSrc, const int32_t* tgtXyz, int nTgt,
+                const int32_t off[3])
+{
+  for (int k = 0; k < 3; k++)
+    if (off[k] <= -(1 << 30) || off[k] >= (1 << 30))
+      return false;
+  int* flag = ex.template alloc<int>(1);
+  ex.zero(flag, sizeof(int));
+  ex.foreach(nSrc, KdCoordCheckFn{srcXyz, flag});
+  ex.foreach(nTgt, KdCoordCheckFn{tgtXyz, flag});
+  int h = 0;
+  ex.download(&h, flag, sizeof(int));
+  return h == 0;
+}
+
 // Recolours numSets attribute sets on the same source and target positions.
-// The grids, both neighbour searches and the backward lists are built once;
-// the forward and final colours of all sets are computed by one launch each,
-// so the launches do not depend on numSets.  sets[s]: srcAttr, A, bitdepth and
-// out (srcXyz / tgtXyz / srcAttr / out: executor memory); refined1 is
-// allocated here.  Returns a PCCB200_* status.
+// The grids (or trees), both neighbour searches and the backward lists are
+// built once; the forward and final colours of all sets are computed by one
+// launch each, so the launches do not depend on numSets.  sets[s]: srcAttr, A,
+// bitdepth and out (srcXyz / tgtXyz / srcAttr / out: executor memory);
+// refined1 is allocated here.  Returns a PCCB200_* status.
 template<class Exec>
 int
 recolour_run(Exec& ex, const pccb200_recolour_params& rp, const int32_t* srcXyz, int nSrc,
              double sourceToTargetScale, const int32_t off[3], const int32_t* tgtXyz, int nTgt,
-             int numSets, const RecolourSet* sets)
+             int numSets, const RecolourSet* sets, RecolourSearch search = kRecolourGrid)
 {
   if (!recolour_args_valid(rp, nSrc, nTgt, sourceToTargetScale, numSets, sets))
     return PCCB200_ERR_INVALID_ARG;
+  const bool exact = search == kRecolourRefExact;
   RecolourConfig cfg;
   const double big = 1.7976931348623157e308;
   cfg.distOffsetFwd = rp.dist_offset_fwd;
@@ -685,10 +735,19 @@ recolour_run(Exec& ex, const pccb200_recolour_params& rp, const int32_t* srcXyz,
 
   ex.phase(0);
   PointGrid gs, gt;
-  int rc = build_point_grid(ex, srcXyz, nSrc, gs);
-  if (rc != PCCB200_OK)
-    return rc;
-  rc = build_point_grid(ex, tgtXyz, nTgt, gt);
+  KdTree ts, tt;
+  int rc;
+  if (exact) {
+    if (!kd_coords_valid(ex, srcXyz, nSrc, tgtXyz, nTgt, off))
+      return PCCB200_ERR_INVALID_ARG;
+    rc = build_kdtree(ex, srcXyz, nSrc, ts);
+    if (rc == PCCB200_OK)
+      rc = build_kdtree(ex, tgtXyz, nTgt, tt);
+  } else {
+    rc = build_point_grid(ex, srcXyz, nSrc, gs);
+    if (rc == PCCB200_OK)
+      rc = build_point_grid(ex, tgtXyz, nTgt, gt);
+  }
   if (rc != PCCB200_OK)
     return rc;
 
@@ -696,22 +755,38 @@ recolour_run(Exec& ex, const pccb200_recolour_params& rp, const int32_t* srcXyz,
   ex.phase(2);
   double* fDist = ex.template alloc<double>(size_t(nTgt) * cfg.kFwd);
   int32_t* fIdx = ex.template alloc<int32_t>(size_t(nTgt) * cfg.kFwd);
-  ex.foreach(nTgt, KnnQueryFn{gs, cfg, tgtXyz, 0, cfg.kFwd, fDist, fIdx});
+  if (exact)
+    ex.foreach(nTgt, KdKnnQueryFn{ts, cfg, tgtXyz, 0, cfg.kFwd, fDist, fIdx});
+  else
+    ex.foreach(nTgt, KnnQueryFn{gs, cfg, tgtXyz, 0, cfg.kFwd, fDist, fIdx});
   int32_t* firstBad = ex.template alloc<int32_t>(1);
   const int32_t never = INT32_MAX;
   ex.upload(firstBad, &never, sizeof(never));
   ex.foreach(nTgt, FirstBadFn{fDist, cfg.kFwd, cfg.maxGeomFwd, firstBad});
-  ForwardColourFn fwd{cfg, fDist, fIdx, firstBad, numSets, {}};
+  RecolourSet withRefined[kRecolourMaxSets];
   for (int s = 0; s < numSets; s++) {
-    fwd.sets[s] = sets[s];
-    fwd.sets[s].refined1 = ex.template alloc<int32_t>(size_t(nTgt) * sets[s].A);
+    withRefined[s] = sets[s];
+    withRefined[s].refined1 = ex.template alloc<int32_t>(size_t(nTgt) * sets[s].A);
   }
-  ex.foreach(nTgt, fwd);
+  if (exact) {
+    ForwardColourT<true> fwd{cfg, fDist, fIdx, firstBad, numSets, {}};
+    for (int s = 0; s < numSets; s++)
+      fwd.sets[s] = withRefined[s];
+    ex.foreach(nTgt, fwd);
+  } else {
+    ForwardColourFn fwd{cfg, fDist, fIdx, firstBad, numSets, {}};
+    for (int s = 0; s < numSets; s++)
+      fwd.sets[s] = withRefined[s];
+    ex.foreach(nTgt, fwd);
+  }
 
   //-- backward: every source in the target, lists per target
   double* bDist = ex.template alloc<double>(size_t(nSrc) * cfg.kBwd);
   int32_t* bIdx = ex.template alloc<int32_t>(size_t(nSrc) * cfg.kBwd);
-  ex.foreach(nSrc, KnnQueryFn{gt, cfg, srcXyz, 1, cfg.kBwd, bDist, bIdx});
+  if (exact)
+    ex.foreach(nSrc, KdKnnQueryFn{tt, cfg, srcXyz, 1, cfg.kBwd, bDist, bIdx});
+  else
+    ex.foreach(nSrc, KnnQueryFn{gt, cfg, srcXyz, 1, cfg.kBwd, bDist, bIdx});
   int* first = ex.template alloc<int>(size_t(nTgt) + 1);
   ex.zero(first, (size_t(nTgt) + 1) * sizeof(int));
   ex.foreach(nSrc, BackwardCountFn{cfg, bDist, bIdx, first});
@@ -725,10 +800,17 @@ recolour_run(Exec& ex, const pccb200_recolour_params& rp, const int32_t* srcXyz,
 
   //-- the colour of every target, every set
   ex.phase(3);
-  FinalColourFn fin{cfg, first, listDist, listSrc, numSets, {}};
-  for (int s = 0; s < numSets; s++)
-    fin.sets[s] = fwd.sets[s];
-  ex.foreach(nTgt, fin);
+  if (exact) {
+    FinalColourT<true> fin{cfg, first, listDist, listSrc, numSets, {}};
+    for (int s = 0; s < numSets; s++)
+      fin.sets[s] = withRefined[s];
+    ex.foreach(nTgt, fin);
+  } else {
+    FinalColourFn fin{cfg, first, listDist, listSrc, numSets, {}};
+    for (int s = 0; s < numSets; s++)
+      fin.sets[s] = withRefined[s];
+    ex.foreach(nTgt, fin);
+  }
   return PCCB200_OK;
 }
 
@@ -737,10 +819,12 @@ template<class Exec>
 int
 recolour_run(Exec& ex, const pccb200_recolour_params& rp, const int32_t* srcXyz,
              const int32_t* srcAttr, int A, int nSrc, double sourceToTargetScale,
-             const int32_t off[3], const int32_t* tgtXyz, int nTgt, int bitdepth, int32_t* out)
+             const int32_t off[3], const int32_t* tgtXyz, int nTgt, int bitdepth, int32_t* out,
+             RecolourSearch search = kRecolourGrid)
 {
   const RecolourSet set{srcAttr, A, bitdepth, nullptr, out};
-  return recolour_run(ex, rp, srcXyz, nSrc, sourceToTargetScale, off, tgtXyz, nTgt, 1, &set);
+  return recolour_run(ex, rp, srcXyz, nSrc, sourceToTargetScale, off, tgtXyz, nTgt, 1, &set,
+                      search);
 }
 
 }  // namespace pccb200

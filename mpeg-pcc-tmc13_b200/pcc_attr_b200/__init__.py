@@ -120,7 +120,8 @@ EXPORTS = [
     "pccb200_profile_reset", "pccb200_quant_weights", "pccb200_quant_weights_fixed",
     "pccb200_quant_weights_scalable", "pccb200_raht_forward", "pccb200_raht_inverse",
     "pccb200_raht_params_default", "pccb200_raht_set_prediction_weights", "pccb200_recolour",
-    "pccb200_recolour_multi", "pccb200_recolour_multi_batch", "pccb200_recolour_multi_batch_dev",
+    "pccb200_recolour_exact", "pccb200_recolour_exact_multi_batch",
+    "pccb200_recolour_exact_multi_batch_dev", "pccb200_recolour_multi", "pccb200_recolour_multi_batch", "pccb200_recolour_multi_batch_dev",
     "pccb200_recolour_multi_dev", "pccb200_recolour_params_default", "pccb200_set_device",
     "pccb200_time_begin", "pccb200_time_end", "pccb200_xyz_to_rpl",
 ]
@@ -425,6 +426,25 @@ def recolour(params, source_xyz, source_attrs, target_xyz, scale=1.0, offset=(0,
     return out
 
 
+def recolour_exact(params, source_xyz, source_attrs, target_xyz, scale=1.0, offset=(0, 0, 0),
+                   bitdepth=8):
+    """as recolour, with the reference's own neighbour search and list order
+    (pccb200_recolour_exact): equal to recolourColour / recolourReflectance bit
+    for bit; coordinates and offsets of |x| < 2^30; -> [n_target, A] int32"""
+    sx = np.ascontiguousarray(source_xyz, dtype=np.int32)
+    sa = np.ascontiguousarray(source_attrs, dtype=np.int32)
+    tx = np.ascontiguousarray(target_xyz, dtype=np.int32)
+    if sa.ndim == 1:
+        sa = sa[:, None]
+    a = sa.shape[1]
+    out = np.zeros((tx.shape[0], a), dtype=np.int32)
+    off = (C.c_int32 * 3)(*[int(v) for v in offset])
+    _check(lib().pccb200_recolour_exact(C.byref(params), _p(sx, C.c_int32), _p(sa, C.c_int32), C.c_int32(a),
+                                        C.c_int32(sx.shape[0]), C.c_double(scale), off, _p(tx, C.c_int32),
+                                        C.c_int32(tx.shape[0]), C.c_int32(bitdepth), _p(out, C.c_int32)))
+    return out
+
+
 def _recolour_batch_args(sources, source_attrs, targets, scales, offsets, outs, bitdepths, ptr):
     """C arrays of a pccb200_recolour_multi_batch(_dev) call; source_attrs[u][s], outs[u][s]"""
     m, k = len(sources), len(source_attrs[0])
@@ -459,10 +479,12 @@ def recolour_multi(params, source_xyz, source_attrs, target_xyz, scale=1.0, offs
     return outs
 
 
-def recolour_multi_batch(params, sources, source_attrs, targets, scales, offsets, bitdepths=None):
+def recolour_multi_batch(params, sources, source_attrs, targets, scales, offsets, bitdepths=None,
+                         exact=False):
     """many units (slices / frames) in one call (pccb200_recolour_multi_batch):
     sources[u] [n_source_u, 3], source_attrs[u][s] [n_source_u, A_s], targets[u],
-    scales[u], offsets[u] (3) -> outs[u][s] [n_target_u, A_s] int32"""
+    scales[u], offsets[u] (3) -> outs[u][s] [n_target_u, A_s] int32.  exact: the
+    reference-exact path (pccb200_recolour_exact_multi_batch)"""
     sources = [np.ascontiguousarray(x, dtype=np.int32) for x in sources]
     targets = [np.ascontiguousarray(x, dtype=np.int32) for x in targets]
     sa = [[np.ascontiguousarray(a, dtype=np.int32).reshape(x.shape[0], -1) for a in u]
@@ -471,15 +493,22 @@ def recolour_multi_batch(params, sources, source_attrs, targets, scales, offsets
     k = len(sa[0])
     args = _recolour_batch_args(sources, sa, targets, scales, offsets, outs, bitdepths or [8] * k,
                                 lambda x: x.ctypes.data)
-    _check(lib().pccb200_recolour_multi_batch(C.byref(params), *args))
+    fn = lib().pccb200_recolour_exact_multi_batch if exact else lib().pccb200_recolour_multi_batch
+    _check(fn(C.byref(params), *args))
     return outs
 
 
+def recolour_exact_multi_batch(params, sources, source_attrs, targets, scales, offsets, bitdepths=None):
+    """recolour_multi_batch on the reference-exact path (pccb200_recolour_exact_multi_batch)"""
+    return recolour_multi_batch(params, sources, source_attrs, targets, scales, offsets, bitdepths, exact=True)
+
+
 def recolour_multi_batch_dev(params, sources, source_attrs, targets, scales, offsets, outs,
-                             bitdepths=None):
+                             bitdepths=None, exact=False):
     """as recolour_multi_batch with contiguous int32 torch CUDA tensors (device
     pointers); the results are written into outs[u][s] [n_target_u, A_s].  The
-    producing stream must be synchronised before the call (see the header)."""
+    producing stream must be synchronised before the call (see the header).
+    exact: the reference-exact path (pccb200_recolour_exact_multi_batch_dev)"""
     tensors = list(sources) + list(targets) + [a for u in source_attrs for a in u] + [o for u in outs for o in u]
     for t in tensors:
         if not (t.is_cuda and t.is_contiguous() and str(t.dtype) == "torch.int32"):
@@ -487,7 +516,16 @@ def recolour_multi_batch_dev(params, sources, source_attrs, targets, scales, off
     k = len(source_attrs[0])
     args = _recolour_batch_args(sources, source_attrs, targets, scales, offsets, outs,
                                 bitdepths or [8] * k, lambda x: x.data_ptr())
-    _check(lib().pccb200_recolour_multi_batch_dev(C.byref(params), *args))
+    fn = lib().pccb200_recolour_exact_multi_batch_dev if exact else lib().pccb200_recolour_multi_batch_dev
+    _check(fn(C.byref(params), *args))
+
+
+def recolour_exact_multi_batch_dev(params, sources, source_attrs, targets, scales, offsets, outs,
+                                   bitdepths=None):
+    """recolour_multi_batch_dev on the reference-exact path
+    (pccb200_recolour_exact_multi_batch_dev)"""
+    recolour_multi_batch_dev(params, sources, source_attrs, targets, scales, offsets, outs, bitdepths,
+                             exact=True)
 
 
 def quant_weights(preds, num_points_in_lod):

@@ -15,10 +15,19 @@ Timed, each after a warm-up call, median of `repeats`:
   (d) pccb200_recolour_multi_batch_dev over the same frames, inputs resident on
       the device (torch CUDA tensors)
 
+  (e) one pccb200_recolour_exact_multi_batch call (both sets), frame 0: the
+      reference-exact path (nanoflann's trees and search) against (b)
+  (f) pccb200_recolour_exact_multi_batch_dev over the same frames, against (d)
+
 Every call synchronises before it returns, so each figure is host wall clock
-around the call; (a) to (c) include the pageable host copies.  The outputs of
-(a) to (d) are compared; the card's name and power limit are printed with the
-numbers."""
+around the call; (a) to (c) and (e) include the pageable host copies.  The
+outputs of (a) to (d) are compared, and those of (e) with (f).  For (b) and
+(e) one more call runs with the library's phase timer on: phase "sort" is the
+grid build or the two tree builds, "block_transform" the searches, forward
+colours and backward lists, "tail" the final colours; the kernel launches of
+one call are counted.  The registers and stack of the tree search kernel
+(ptxas, from the library's build log) and the card's name and power limit are
+printed with the numbers."""
 import json
 import os
 import subprocess
@@ -92,13 +101,47 @@ def main():
         out[key] = {"ms_median": med, "ms_min": best}
         if "batch" in key:
             out[key]["ms_per_frame"] = med / frames
+    def exact():
+        res["e"] = pb.recolour_exact_multi_batch(rp, [src[0]], [attrs[0]], [tgt[0]], [0.5], [(0, 0, 0)], bds)[0]
+
+    eouts = [[torch.empty_like(o) for o in u] for u in douts]
+
+    def exact_dev():
+        pb.recolour_exact_multi_batch_dev(rp, dsrc, dattrs, dtgt, scales, offs, eouts, bds)
+
+    for key, fn in (("e_exact_multi_batch_1_frame", exact), (f"f_exact_multi_batch_dev_{frames}_frames", exact_dev)):
+        med, best = timed(fn, repeats)
+        out[key] = {"ms_median": med, "ms_min": best}
+        if "dev" in key:
+            out[key]["ms_per_frame"] = med / frames
+
+    # per-phase device time and launches of one call, grid (b) and exact (e)
+    for key, fn in (("phases_b_grid", multi), ("phases_e_exact", exact)):
+        pb.profile_reset()
+        pb.profile_enable(True)
+        before = pb.kernel_launch_count()
+        fn()
+        launches = pb.kernel_launch_count() - before
+        pb.profile_enable(False)
+        prof = pb.profile_read()
+        out[key] = {"launches": int(launches),
+                    "ms": {n: round(v[0], 3) for n, v in prof.items() if v[1]}}
+    log = os.path.join(ROOT, "mpeg-pcc-tmc13_b200", "build.log")
+    if os.path.exists(log):
+        lines = open(log).read().splitlines()
+        for i, l in enumerate(lines):
+            if "k_foreachINS_12KdKnnQueryFn" in l and "Compiling entry" in l:
+                out["ptxas_KdKnnQueryFn"] = " | ".join(x.strip() for x in lines[i + 1:i + 3])
     dres = [[o.cpu().numpy() for o in u] for u in douts]
+    eres = [[o.cpu().numpy() for o in u] for u in eouts]
+    out["exact_batch_equals_exact_call"] = all(np.array_equal(x, y) for x, y in zip(res["e"], eres[0]))
+    out["exact_differs_from_grid_targets"] = int(sum((x != y).any(axis=1).sum() for x, y in zip(res["e"], res["b"])))
     same = (all(np.array_equal(x, y) for x, y in zip(res["a"], res["b"]))
             and all(np.array_equal(x, y) for x, y in zip(res["a"], res["c"][0]))
             and all(np.array_equal(x, y) for u, v in zip(res["c"], dres) for x, y in zip(u, v)))
     out["outputs_identical"] = bool(same)
     print(json.dumps(out, indent=1))
-    sys.exit(0 if same else 1)
+    sys.exit(0 if same and out["exact_batch_equals_exact_call"] else 1)
 
 
 if __name__ == "__main__":
