@@ -687,6 +687,32 @@ typedef struct pccb200_lod_handle_s* pccb200_lod_handle;
  * never needs them). */
 int pccb200_lod_create(const pccb200_lod_params* params, const int32_t* xyz, int32_t n,
                        pccb200_lod_handle* handle_out);
+/* A handle over levels of detail the caller already holds (pcc::AttributeLods
+ * after AttributeLods::generate, whoever built them), so that the lifting entries
+ * below code on them unchanged.
+ *   preds[n], indexes[n]   predictor order, as pccb200_lod_build returns them
+ *   num_points_in_lod      lod_count cumulative counts, the last one n
+ *   num_detail_levels      aps.maxNumDetailLevels(): the length of the LCP rows
+ *                          (num_detail_levels_minus1 + 1, or 21 with scalable
+ *                          lifting); lod_count..PCCB200_MAX_LODS
+ *   scal                   NULL, or scalable lifting: the quantisation weights are
+ *                          then computeQuantizationWeightsScalable with
+ *                          (geom_num_points, min_geom_node_size_log2) of scal, the
+ *                          encoder's (0 or n, 0) or the decoder's; max_neigh_range
+ *                          is not read
+ * Host checks, before any device lookup, return PCCB200_ERR_INVALID_ARG: null
+ * pointers, n <= 0, lod_count outside 1..PCCB200_MAX_LODS, counts that decrease
+ * (equal neighbours are an empty level, which the reference's scalable levels
+ * have) or start at 0, a last count other than n, num_detail_levels out of
+ * range, and a malformed scal.  On the device: indexes that are not a
+ * permutation of [0, n), or a predictor with more than three neighbours or one
+ * outside [0, n), return PCCB200_ERR_INVALID_ARG too.  Predictors that reference
+ * their own level of detail are refused by the lifting calls
+ * (PCCB200_ERR_UNSUPPORTED).  pccb200_lod_reusable is 0 for such a handle. */
+int pccb200_lod_import(const pccb200_predictor* preds, const uint32_t* indexes, int32_t n,
+                       const uint32_t* num_points_in_lod, int32_t lod_count,
+                       int32_t num_detail_levels, const pccb200_lod_scalable* scal,
+                       pccb200_lod_handle* handle_out);
 void pccb200_lod_destroy(pccb200_lod_handle handle);
 /* 1 if LoDs built with the handle's parameters serve `params` as well (the
  * comparisons of AttributeLods::isReusable that this structure carries), else 0. */

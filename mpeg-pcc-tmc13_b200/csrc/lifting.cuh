@@ -63,6 +63,45 @@ struct LodCheckFn {
   }
 };
 
+PCC_HD int
+atomic_add_old_i32(int* p, int v)
+{
+#if defined(__CUDA_ARCH__)
+  return atomicAdd(p, v);
+#else
+  const int old = *p;
+  *p += v;
+  return old;
+#endif
+}
+
+// levels of detail made by the caller (pccb200_lod_import), entry i of total:
+// flag bit 0: indexes is not a permutation of [0, total) (an entry out of
+// range, or one met twice; seen: total zeroed counters); bit 1: a predictor is
+// malformed, as in LodCheckFn.  Both would turn the lifting gathers and
+// scatters into out-of-bounds or racing accesses.
+struct LodImportCheckFn {
+  const pccb200_predictor* preds;
+  const uint32_t* indexes;
+  int* seen;
+  int* flag;
+  int64_t total;
+  PCC_HD void operator()(int64_t i) const
+  {
+    const int64_t k = indexes[i];
+    if (k >= total || atomic_add_old_i32(&seen[k], 1) != 0)
+      atomic_or_i32(flag, 1);
+    const pccb200_predictor& p = preds[i];
+    if (p.neighbor_count > 3) {
+      atomic_or_i32(flag, 2);
+      return;
+    }
+    for (uint32_t j = 0; j < p.neighbor_count; j++)
+      if (int64_t(p.predictor_index[j]) >= total)
+        atomic_or_i32(flag, 2);
+  }
+};
+
 // neighbour weight j of a predictor: its own (lifting, PCCTMC3Common.h:828-854)
 // or the fixed per-slot weight of the predicting transform
 // (computeQuantizationWeights, PCCTMC3Common.h:895-921)
@@ -444,6 +483,21 @@ run_quant_weights(Exec& ex, const pccb200_predictor* preds, int64_t n,
       ex.foreach(e - s, QuantWeightLodFn{preds, qw, s, nw});
   }
   return PCCB200_OK;
+}
+
+// PCCB200_ERR_INVALID_ARG unless indexes[n] is a permutation of [0, n) and
+// every predictor has at most three neighbours, all of them in [0, n)
+template<class Exec>
+int
+run_lod_import_check(Exec& ex, const pccb200_predictor* preds, const uint32_t* indexes, int64_t n)
+{
+  int* seen = ex.template alloc<int>(size_t(n) + 1);
+  ex.zero(seen, (size_t(n) + 1) * sizeof(int));
+  int* dFlag = seen + n;
+  ex.foreach(n, LodImportCheckFn{preds, indexes, seen, dFlag, n});
+  int flag = 0;
+  ex.download(&flag, dFlag, sizeof(int));
+  return flag ? PCCB200_ERR_INVALID_ARG : PCCB200_OK;
 }
 
 template<class Exec>

@@ -49,6 +49,11 @@ struct pccb200_lod_handle_s {
   // the handle (a handle made for the predicting transform never needs them)
   std::mutex qwMu;
   bool qwReady = false;
+  // made by pccb200_lod_import from the caller's levels of detail: never
+  // reusable, and with scalable set its weights are the scalable ones of scal
+  bool imported = false;
+  bool scalable = false;
+  pccb200_lod_scalable scal = {};
 };
 
 namespace pccb200 {
@@ -719,7 +724,12 @@ code_lift(bool forward, const std::vector<LiftUnit>& units, bool nameUnits)
       if (h) {
         std::lock_guard<std::mutex> g(h->qwMu);
         if (!h->qwReady) {
-          int rcq = run_quant_weights(ex, h->st.preds, u.n, h->st.npl, h->st.lodCount, h->st.qw);
+          const uint64_t geomPoints = h->scal.geom_num_points ? h->scal.geom_num_points : u.n;
+          int rcq = h->scalable
+                      ? run_quant_weights_scalable(ex, h->st.npl, h->st.lodCount, geomPoints,
+                                                   h->scal.min_geom_node_size_log2, u.n, h->st.qw)
+                      : run_quant_weights(ex, h->st.preds, u.n, h->st.npl, h->st.lodCount,
+                                          h->st.qw);
           if (rcq != PCCB200_OK)
             return fail(rcq, unit + "invalid levels of detail");
           PCC_CUDA_CHECK(cudaStreamSynchronize(ex.stream));  // other lanes read them from now on
@@ -1554,6 +1564,70 @@ pccb200_lod_create(const pccb200_lod_params* params, const int32_t* xyz, int32_t
   return PCCB200_OK;
 }
 
+int
+pccb200_lod_import(const pccb200_predictor* preds, const uint32_t* indexes, int32_t n,
+                   const uint32_t* num_points_in_lod, int32_t lod_count,
+                   int32_t num_detail_levels, const pccb200_lod_scalable* scal,
+                   pccb200_lod_handle* handle_out)
+{
+  if (handle_out)
+    *handle_out = nullptr;
+  if (!preds || !indexes || !num_points_in_lod || !handle_out || n <= 0)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  if (lod_count < 1 || lod_count > PCCB200_MAX_LODS)
+    return fail(PCCB200_ERR_INVALID_ARG, "lod_count outside 1..PCCB200_MAX_LODS");
+  for (int l = 0; l < lod_count; l++)
+    if (num_points_in_lod[l] < (l ? num_points_in_lod[l - 1] : 1u))
+      return fail(PCCB200_ERR_INVALID_ARG, "num_points_in_lod is not increasing");
+  if (num_points_in_lod[lod_count - 1] != uint32_t(n))
+    return fail(PCCB200_ERR_INVALID_ARG, "the last count of num_points_in_lod is not n");
+  if (num_detail_levels < lod_count || num_detail_levels > PCCB200_MAX_LODS)
+    return fail(PCCB200_ERR_INVALID_ARG, "num_detail_levels outside lod_count..PCCB200_MAX_LODS");
+  if (scal && (scal->reserved != 0 || scal->min_geom_node_size_log2 < 0
+               || scal->min_geom_node_size_log2 >= kScalableLevels
+               || (scal->geom_num_points != 0 && scal->geom_num_points < n)))
+    return fail(PCCB200_ERR_INVALID_ARG,
+                "reserved not 0, min_geom_node_size_log2 out of range or geom_num_points < n");
+  pccb200_lod_handle h = new (std::nothrow) pccb200_lod_handle_s();
+  if (!h)
+    return fail(PCCB200_ERR_NOMEM, "host allocation failed");
+  h->params.num_detail_levels = num_detail_levels;
+  h->imported = true;
+  h->scalable = scal != nullptr;
+  if (scal)
+    h->scal = *scal;
+  h->st.n = n;
+  h->st.numDetailLevels = num_detail_levels;
+  h->st.lodCount = lod_count;
+  for (int l = 0; l < lod_count; l++)
+    h->st.npl[l] = num_points_in_lod[l];
+  int rc = with_device([&](DeviceExec& ex) -> int {
+    h->device = ctx().device;
+    const size_t szP = (size_t(n) * sizeof(pccb200_predictor) + 255) & ~size_t(255);
+    const size_t szQ = (size_t(n) * sizeof(uint64_t) + 255) & ~size_t(255);
+    const size_t szI = (size_t(n) * sizeof(uint32_t) + 255) & ~size_t(255);
+    PCC_CUDA_CHECK(cudaMalloc(&h->block, szP + szQ + szI));
+    char* b = static_cast<char*>(h->block);
+    h->st.preds = reinterpret_cast<pccb200_predictor*>(b);
+    h->st.qw = reinterpret_cast<uint64_t*>(b + szP);
+    h->st.idx = reinterpret_cast<uint32_t*>(b + szP + szQ);
+    ex.upload(h->st.preds, preds, size_t(n) * sizeof(pccb200_predictor));
+    ex.upload(h->st.idx, indexes, size_t(n) * sizeof(uint32_t));
+    if (run_lod_import_check(ex, h->st.preds, h->st.idx, n) != PCCB200_OK)
+      return fail(PCCB200_ERR_INVALID_ARG,
+                  "indexes is not a permutation of [0, n) or a predictor is malformed");
+    return PCCB200_OK;
+  });
+  if (rc != PCCB200_OK) {
+    if (h->block)
+      cudaFree(h->block);
+    delete h;
+    return rc;
+  }
+  *handle_out = h;
+  return PCCB200_OK;
+}
+
 void
 pccb200_lod_destroy(pccb200_lod_handle handle)
 {
@@ -1569,7 +1643,7 @@ pccb200_lod_destroy(pccb200_lod_handle handle)
 int
 pccb200_lod_reusable(pccb200_lod_handle h, const pccb200_lod_params* p)
 {
-  if (!h || !p)
+  if (!h || !p || h->imported)
     return 0;
   const pccb200_lod_params& a = h->params;
   // the order of AttributeLods::isReusable (tmc3/AttributeCommon.cpp:76-140)

@@ -20,6 +20,7 @@
 #include "RAHT.h"
 
 #include "pcc_attr_b200.h"
+#include "qpset_flatten.h"
 
 namespace pcc {
 
@@ -42,23 +43,7 @@ flatten(const RahtPredictionParams& rp, const QpSet& qs, bool rahtExtension,
       i < int(rp.predWeightChild.size()) ? rp.predWeightChild[i] : 0;
   p.raht_extension = rahtExtension;
 
-  if (qs.layers.empty() || int(qs.layers.size()) > PCCB200_MAX_QP_LAYERS
-      || int(qs.rahtAcCoeffQps.size()) > PCCB200_MAX_AC_QP_LAYERS)
-    throw std::runtime_error("pcc_attr_b200: unsupported number of qp layers");
-  q = pccb200_qpset{};
-  q.num_layers = int(qs.layers.size());
-  for (int i = 0; i < q.num_layers; i++) {
-    q.layers[i][0] = qs.layers[i][0];
-    q.layers[i][1] = qs.layers[i][1];
-  }
-  q.max_qp = qs.maxQp;
-  q.fixed_point_qp_offset = qs.fixedPointQpOffset;
-  q.num_ac_coeff_qp_layers = int(qs.rahtAcCoeffQps.size());
-  for (int l = 0; l < q.num_ac_coeff_qp_layers; l++)
-    for (int c = 0; c < 7; c++) {
-      q.ac_coeff_qps[l][c][0] = qs.rahtAcCoeffQps[l][c][0];
-      q.ac_coeff_qps[l][c][1] = qs.rahtAcCoeffQps[l][c][1];
-    }
+  flatten_qpset(qs, q);
 }
 
 // Qps is std::array<int, 2>: the per-point offsets are already a contiguous

@@ -115,7 +115,7 @@ EXPORTS = [
     "pccb200_last_error", "pccb200_lift_dequantize", "pccb200_lift_forward",
     "pccb200_lift_inverse", "pccb200_lift_quantize", "pccb200_lod_build",
     "pccb200_lod_build_scalable", "pccb200_lod_create",
-    "pccb200_lod_destroy", "pccb200_lod_info", "pccb200_lod_reusable", "pccb200_morton_sort",
+    "pccb200_lod_destroy", "pccb200_lod_import", "pccb200_lod_info", "pccb200_lod_reusable", "pccb200_morton_sort",
     "pccb200_offset_and_scale", "pccb200_profile_enable", "pccb200_profile_read",
     "pccb200_profile_reset", "pccb200_quant_weights", "pccb200_quant_weights_fixed",
     "pccb200_quant_weights_scalable", "pccb200_raht_forward", "pccb200_raht_inverse",
@@ -630,6 +630,60 @@ def lod_build_scalable(params, scal, xyz):
         C.cast(preds.ctypes.data, C.POINTER(Predictor)), _p(indexes, C.c_uint32),
         _p(npl, C.c_uint32), C.byref(cnt)))
     return preds, indexes, npl[:cnt.value].copy()
+
+
+def lod_import(preds, indexes, num_points_in_lod, num_detail_levels, scal=None):
+    """pccb200_lod_import: a level-of-detail handle over levels of detail the
+    caller holds (preds: PREDICTOR_DTYPE [N], indexes [N], cumulative counts;
+    scal: LodScalable for scalable lifting, or None) -> handle (an int);
+    release it with lod_destroy"""
+    preds = np.ascontiguousarray(preds, dtype=PREDICTOR_DTYPE)
+    indexes = np.ascontiguousarray(indexes, dtype=np.uint32)
+    npl = np.ascontiguousarray(num_points_in_lod, dtype=np.uint32)
+    h = C.c_void_p()
+    _check(lib().pccb200_lod_import(
+        C.cast(preds.ctypes.data, C.POINTER(Predictor)), _p(indexes, C.c_uint32),
+        C.c_int32(len(preds)), _p(npl, C.c_uint32), C.c_int32(len(npl)),
+        C.c_int32(num_detail_levels), C.byref(scal) if scal is not None else None, C.byref(h)))
+    return h.value
+
+
+def lod_destroy(handle):
+    lib().pccb200_lod_destroy(C.c_void_p(handle))
+
+
+def attr_lift_encode_lod(handle, qpset, attrs, lcp_enabled=0, bitdepth=8, qpoffs=None):
+    """pccb200_attr_lift_encode_lod -> (values [N,A] coding order, reconstruction
+    [N,A] point order, lcp row of MAX_LODS entries)"""
+    attrs = np.ascontiguousarray(attrs, dtype=np.int32).copy()
+    n, a = attrs.shape
+    values = np.zeros((n, a), dtype=np.int32)
+    lcp = np.zeros(MAX_LODS, dtype=np.int8)
+    if qpoffs is not None:
+        qpoffs = np.ascontiguousarray(qpoffs, dtype=np.int32)
+    _check(lib().pccb200_attr_lift_encode_lod(
+        C.c_void_p(handle), C.byref(qpset), C.c_int32(lcp_enabled), _p(qpoffs, C.c_int32),
+        _p(attrs, C.c_int32), C.c_int32(a), C.c_int32(bitdepth), _p(values, C.c_int32),
+        _p(lcp, C.c_int8)))
+    return values, attrs, lcp
+
+
+def attr_lift_decode_lod(handle, qpset, values, lcp=None, bitdepth=8, qpoffs=None):
+    """pccb200_attr_lift_decode_lod -> reconstruction [N,A] point order"""
+    values = np.ascontiguousarray(values, dtype=np.int32)
+    n, a = values.shape
+    attrs = np.zeros((n, a), dtype=np.int32)
+    l2 = None
+    if lcp is not None:
+        l2 = np.zeros(MAX_LODS, dtype=np.int8)
+        l2[:len(lcp)] = lcp
+    if qpoffs is not None:
+        qpoffs = np.ascontiguousarray(qpoffs, dtype=np.int32)
+    _check(lib().pccb200_attr_lift_decode_lod(
+        C.c_void_p(handle), C.byref(qpset), C.c_int32(1 if lcp is not None else 0),
+        _p(qpoffs, C.c_int32), _p(attrs, C.c_int32), C.c_int32(a), C.c_int32(bitdepth),
+        _p(values, C.c_int32), _p(l2, C.c_int8)))
+    return attrs
 
 
 def attr_lift_encode(lod_params, qpset, xyz, attrs, lcp_enabled=0, bitdepth=8, qpoffs=None):
