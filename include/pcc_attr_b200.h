@@ -953,6 +953,76 @@ int pccb200_estimate_dist2(const int32_t* xyz, int32_t n, int32_t sampling_perio
                            int32_t search_range, float percentile_estimate,
                            int32_t* shift_bits_out);
 
+/* Predicting transform decoder (attr_encoding 0, transformType 1) -------------
+ *
+ * AttributeDecoder::decode{Colors,Reflectances}Pred
+ * (tmc3/AttributeDecoder.cpp:328-391,446-523) after its entropy decoding:
+ * values_in holds, per point in coding (predictor) order, the values the
+ * reference's loop decodes (zero runs expanded: decodeRunLength / decode),
+ * with the prediction mode still in their low bits.  The library applies the
+ * rest of the loop: fixed-weight quantisation weights (quant_neigh_weight),
+ * the quantisers of the point's level (quantLayer) and qp offsets, the mode's
+ * eligibility from the neighbours' reconstructed values against
+ * adaptive_prediction_threshold << max(0, bitdepth - 8), the mode unpacked
+ * from the values, the prediction, dequantisation, inter-component prediction
+ * and the clip to [0, 2^bitdepth - 1].  The output is the decoded attribute
+ * per point, in point order, bit-identical to the reference's.
+ *
+ * A point's prediction reads the reconstructions of its neighbours, whose
+ * predictor indexes must be below its own (the levels of detail of the
+ * predicting transform have that form, also with intra-LoD prediction).
+ * Predictors that break it return PCCB200_ERR_INVALID_ARG before any decoding
+ * starts.  Scalable lifting handles and inter-frame prediction are not
+ * supported (PCCB200_ERR_UNSUPPORTED for a scalable handle).
+ *
+ * qpset: fixed_point_qp_offset 0, as deriveQpSet sets it for this transform.
+ * point_qp_offsets: N x 2 in point order (the region offsets of
+ * QpSet::quantizers), or NULL.  icp_coeffs: a host row of PCCB200_MAX_LODS
+ * triplets, abh.icpCoeffs per level of detail, or NULL when the brick header
+ * carries none (icpPresent false). */
+typedef struct pccb200_pred_params {
+  int32_t max_num_direct_predictors;      /* 0..3 */
+  int32_t direct_avg_predictor_disabled;  /* direct_avg_predictor_disabled_flag */
+  int32_t adaptive_prediction_threshold;  /* unscaled, as in the APS */
+  int32_t icp_enabled;                    /* inter_component_prediction_enabled_flag */
+} pccb200_pred_params;
+
+#define PCCB200_MAX_PRED_SETS 4
+
+/* On a pccb200_lod_create / pccb200_lod_import handle: one attribute of
+ * num_attrs (1 or 3) components.  values_in, attrs_out: N x num_attrs. */
+int pccb200_attr_pred_decode_lod(pccb200_lod_handle handle, const pccb200_qpset* qpset,
+                                 const pccb200_pred_params* pred,
+                                 const int32_t quant_neigh_weight[3],
+                                 const int32_t* point_qp_offsets, const int8_t* icp_coeffs,
+                                 const int32_t* values_in, int32_t num_attrs, int32_t bitdepth,
+                                 int32_t* attrs_out);
+
+/* num_units units (slices or frames), each with its own LoD parameters
+ * lods[u] (pred_weight_blending and the intra-LoD settings included),
+ * positions xyz[u] (n[u] x 3), quant_neigh_weight[3u..3u+2] and qp offsets
+ * point_qp_offsets[u] (or point_qp_offsets NULL, or an entry NULL), and
+ * num_sets (1..PCCB200_MAX_PRED_SETS) attribute sets sharing its levels of
+ * detail.  qpsets[s], pred[s], num_attrs[s], bitdepths[s] are per set;
+ * values_in[u * num_sets + s], icp_coeffs[u * num_sets + s] (or icp_coeffs
+ * NULL, or an entry NULL) and attrs_out[u * num_sets + s] per unit and set.
+ * Units are spread over the library's lanes; the units of a lane decode in one
+ * dataflow launch.  Results are bit-identical to one call per unit.
+ * The _dev entry takes device pointers for xyz, point_qp_offsets, values_in and
+ * attrs_out; everything else stays on the host. */
+int pccb200_attr_pred_decode_multi_batch(
+  int32_t num_units, const pccb200_lod_params* const* lods, const int32_t* quant_neigh_weight,
+  int32_t num_sets, const pccb200_qpset* const* qpsets, const pccb200_pred_params* pred,
+  const int32_t* num_attrs, const int32_t* bitdepths, const int32_t* const* xyz, const int32_t* n,
+  const int32_t* const* point_qp_offsets, const int32_t* const* values_in,
+  const int8_t* const* icp_coeffs, int32_t* const* attrs_out);
+int pccb200_attr_pred_decode_multi_batch_dev(
+  int32_t num_units, const pccb200_lod_params* const* lods, const int32_t* quant_neigh_weight,
+  int32_t num_sets, const pccb200_qpset* const* qpsets, const pccb200_pred_params* pred,
+  const int32_t* num_attrs, const int32_t* bitdepths, const int32_t* const* d_xyz,
+  const int32_t* n, const int32_t* const* d_point_qp_offsets, const int32_t* const* d_values_in,
+  const int8_t* const* icp_coeffs, int32_t* const* d_attrs_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,39 @@ k_ordered(F f, int64_t n, unsigned long long* ticket)
   }
 }
 
+// Warp-uniform dataflow over a gang of chains: CTA b serves chain
+// items[b % numItems] (as k_block_warp_gang serves units).  Each warp claims
+// 32 consecutive tickets of its chain (item.ticket, item.size() of them);
+// item(t) returns false while ticket t waits for a lower ticket of the same
+// chain.  Lanes of a warp never spin against each other: the ready ones run,
+// and the warp repeats (the k_cell_levels pattern).  Lower tickets are held
+// by running warps, so any grid is free of deadlock.
+template<class F>
+__global__ void __launch_bounds__(256)
+k_warp_flow(const F* __restrict__ items, int numItems)
+{
+  const F& f = items[blockIdx.x % numItems];
+  const int64_t n = f.size();
+  const int lane = threadIdx.x & 31;
+  for (;;) {
+    unsigned long long base = 0;
+    if (lane == 0)
+      base = atomicAdd(f.ticket, 32ull);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (base >= (unsigned long long)n)
+      return;
+    const int64_t t = int64_t(base) + lane;
+    bool done = t >= n;
+    while (__any_sync(0xffffffffu, !done)) {
+      bool progress = false;
+      if (!done && f(t))
+        done = progress = true;
+      if (!__any_sync(0xffffffffu, progress))
+        __nanosleep(40);
+    }
+  }
+}
+
 constexpr int kTileThreads = 256;
 constexpr int kTileItems = 8;
 constexpr int kTile = kTileThreads * kTileItems;
@@ -423,6 +456,41 @@ struct DeviceExec {
       blocks = cap;
     Scope sc(*this);
     k_ordered<F><<<unsigned(blocks), kOrderedThreads, 0, stream>>>(f, n, ticket);
+    g_launchCount++;
+    PCC_CUDA_CHECK(cudaGetLastError());
+  }
+
+  // One k_warp_flow launch over numItems chains: hItems on the host, dItems
+  // the same in executor memory, their tickets zeroed.  The persistent grid
+  // is the resident CTAs of the machine shared among the calls in flight, a
+  // multiple of the number of chains, and no more than their items need.
+  template<class F>
+  void flow(const F* hItems, const F* dItems, int numItems)
+  {
+    if (numItems <= 0)
+      return;
+    static const int perSM = [] {
+      int v = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, k_warp_flow<F>, 256, 0) != cudaSuccess)
+        v = 0;
+      return v < 1 ? 1 : v;
+    }();
+    int64_t cap = int64_t(numSMs) * perSM;
+    const int inFlight = activeCalls ? activeCalls->load() : 1;
+    if (inFlight > 1)
+      cap /= inFlight;
+    int64_t perChain = 1;
+    for (int c = 0; c < numItems; c++) {
+      const int64_t want = (hItems[c].size() + 255) / 256;
+      perChain = want > perChain ? want : perChain;
+    }
+    int64_t fit = cap / numItems;
+    if (fit < 1)
+      fit = 1;
+    if (perChain > fit)
+      perChain = fit;
+    Scope sc(*this);
+    k_warp_flow<F><<<unsigned(perChain * numItems), 256, 0, stream>>>(dItems, numItems);
     g_launchCount++;
     PCC_CUDA_CHECK(cudaGetLastError());
   }

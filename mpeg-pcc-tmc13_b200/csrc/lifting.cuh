@@ -12,8 +12,8 @@
 // scatter-adds of the update step and of the quantisation weights are 64-bit
 // integer atomics: addition modulo 2^64 is order independent, so the results
 // are bit-identical to the sequential walk.  A predictor that references its
-// own LoD is reported through an error word and executed by a single ordered
-// thread instead.
+// own LoD is reported through an error word; the quantisation weights of such
+// a level are a counter-driven dataflow on the device (QwFlowFn).
 #pragma once
 
 #include <vector>
@@ -41,7 +41,8 @@ struct FillU64Fn {
 
 // flag bit 0: a predictor in [start, start + n) references an index >= start
 // (its own level of detail); bit 1: a predictor is malformed (more than three
-// neighbours, or an index outside [0, total))
+// neighbours, or an index outside [0, total)); bit 2 (with bit 0): it
+// references an index not below its own
 struct LodCheckFn {
   const pccb200_predictor* preds;
   int64_t start;
@@ -57,6 +58,8 @@ struct LodCheckFn {
     for (uint32_t j = 0; j < p.neighbor_count; j++) {
       if (int64_t(p.predictor_index[j]) >= total)
         atomic_or_i32(flag, 2);
+      else if (int64_t(p.predictor_index[j]) >= start + i)
+        atomic_or_i32(flag, 5);
       else if (int64_t(p.predictor_index[j]) >= start)
         atomic_or_i32(flag, 1);
     }
@@ -144,6 +147,88 @@ struct QuantWeightSeqFn {
     }
   }
 };
+
+// The same walk of a level [s, e) that references itself, as a dataflow over
+// the level: cnt[i - s] counts the referrers of predictor i inside the level
+// (QwReferrerCountFn).  Ticket t is predictor e - 1 - t.  Once its counter is
+// 0, every contribution to its weight has been added (the referrers of a
+// predictor have higher indexes); it adds its own to each neighbour, then --
+// after a release fence -- decrements the counters of the neighbours inside
+// the level.  Each contribution depends on a final weight only, and uint64
+// addition commutes, so the weights equal QuantWeightSeqFn's bit for bit.
+struct QwReferrerCountFn {
+  const pccb200_predictor* preds;
+  int* cnt;
+  int64_t start;
+  PCC_HD void operator()(int64_t i) const
+  {
+    const pccb200_predictor& p = preds[start + i];
+    for (uint32_t j = 0; j < p.neighbor_count; j++)
+      if (int64_t(p.predictor_index[j]) >= start)
+        atomic_add_old_i32(&cnt[p.predictor_index[j] - start], 1);
+  }
+};
+
+struct QwFlowFn {
+  const pccb200_predictor* preds;
+  uint64_t* qw;
+  int* cnt;
+  int64_t start, end;
+  NeighWeights nw;
+  unsigned long long* ticket;  // of the dataflow launch
+  PCC_HD int64_t size() const { return end - start; }
+  // false while a referrer of the predictor has not run yet
+  PCC_HD bool operator()(int64_t t) const
+  {
+    const int64_t i = end - 1 - t;
+#if defined(__CUDA_ARCH__)
+    int c;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(c) : "l"(cnt + (i - start)) : "memory");
+    if (c)
+      return false;
+    __threadfence();
+    unsigned long long w;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(qw + i) : "memory");
+#else
+    if (cnt[i - start])
+      return false;
+    const uint64_t w = qw[i];
+#endif
+    const pccb200_predictor& p = preds[i];
+    for (uint32_t j = 0; j < p.neighbor_count; j++)
+      atomic_add_u64(&qw[p.predictor_index[j]], div_exp2_round_half_inf_u(nw.of(p, j) * w, 8));
+#if defined(__CUDA_ARCH__)
+    __threadfence();
+#endif
+    for (uint32_t j = 0; j < p.neighbor_count; j++)
+      if (int64_t(p.predictor_index[j]) >= start)
+        atomic_add_old_i32(&cnt[p.predictor_index[j] - start], -1);
+    return true;
+  }
+};
+
+// A level that references itself: the counter-driven QwFlowFn on an executor
+// with a dataflow launch (the device), QuantWeightSeqFn in one thread on any
+// other (the host emulation, where it is the check of the dataflow).
+template<class Exec>
+auto
+quant_weights_self(Exec& ex, QwFlowFn f, int) -> decltype(ex.flow(&f, &f, 1), void())
+{
+  ex.zero(f.cnt, size_t(f.end - f.start) * sizeof(int));
+  ex.foreach(f.end - f.start, QwReferrerCountFn{f.preds, f.cnt, f.start});
+  f.ticket = ex.template alloc<unsigned long long>(1);
+  ex.zero(f.ticket, sizeof(unsigned long long));
+  QwFlowFn* d = ex.template alloc<QwFlowFn>(1);
+  ex.upload(d, &f, sizeof(f));
+  ex.flow(&f, d, 1);
+}
+
+template<class Exec>
+void
+quant_weights_self(Exec& ex, const QwFlowFn& f, long)
+{
+  ex.foreach(1, QuantWeightSeqFn{f.preds, f.qw, f.start, f.end, f.nw});
+}
 
 // computeQuantizationWeightsScalable (PCCTMC3Common.h:858-891): one constant
 // per level of detail
@@ -474,12 +559,18 @@ run_quant_weights(Exec& ex, const pccb200_predictor* preds, int64_t n,
   for (int l = 0; l < lodCount; l++)
     if (flags[l] & 2)
       return PCCB200_ERR_INVALID_ARG;
+  int* cnt = nullptr;
   for (int l = lodCount - 1; l >= 0; l--) {
     int64_t s = l ? numPointsInLod[l - 1] : 0;
     int64_t e = numPointsInLod[l];
-    if (flags[l])
+    // (a reference to a higher index has no dataflow order: one ordered walk)
+    if (flags[l] & 4) {
       ex.foreach(1, QuantWeightSeqFn{preds, qw, s, e, nw});
-    else
+    } else if (flags[l]) {
+      if (!cnt)
+        cnt = ex.template alloc<int>(size_t(n));
+      quant_weights_self(ex, QwFlowFn{preds, qw, cnt, s, e, nw, nullptr}, 0);
+    } else
       ex.foreach(e - s, QuantWeightLodFn{preds, qw, s, nw});
   }
   return PCCB200_OK;

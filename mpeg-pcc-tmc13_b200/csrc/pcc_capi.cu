@@ -30,6 +30,7 @@
 #include "lifting.cuh"
 #include "lift_pipeline.cuh"
 #include "lod_pipeline.cuh"
+#include "pred_pipeline.cuh"
 #include "morton_sort.cuh"
 #include "pcc_attr_b200.h"
 #include "raht_pipeline.cuh"
@@ -1010,6 +1011,130 @@ recolour_multi(bool dev, const pccb200_recolour_params* params, int numSets, int
   if (rc != PCCB200_OK)
     return rc;
   return code_recolour(*params, units, true);
+}
+
+// One unit of a predicting-transform decode: the handle's levels of detail, or
+// lod and xyz; qp offsets ([n, 2]) or null; per set the caller's values_in and
+// attrs_out ([n, A]) and ICP row.  dev: device pointers, otherwise host ones.
+struct PredCallUnit {
+  int n = 0;
+  const int32_t* xyz = nullptr;
+  const int32_t* qpo = nullptr;
+  const pccb200_lod_params* lod = nullptr;
+  pccb200_lod_handle handle = nullptr;
+  PredUnit pu = {};
+};
+
+// Validated units dealt over at most kCallLanes lanes (unit u to lane
+// u % lanes); the units of a lane form one gang: levels of detail, then one
+// attr_pred_decode_on_lods (one dataflow launch) for all of them.
+int
+code_pred(bool dev, const std::vector<PredCallUnit>& units)
+{
+  const int numUnits = int(units.size());
+  const int lanes = numUnits < kCallLanes ? numUnits : kCallLanes;
+  return parallel_for(lanes, lanes, [&](int g) -> int {
+    std::vector<int> mine;
+    for (int u = g; u < numUnits; u += lanes)
+      mine.push_back(u);
+    for (int u : mine)
+      if (units[u].handle && units[u].handle->device != ctx().device)
+        return fail(PCCB200_ERR_INVALID_ARG, "unit " + std::to_string(u)
+                                               + ": handle belongs to another device");
+    return with_device([&](DeviceExec& ex) -> int {
+      std::vector<LodState> st(mine.size());
+      std::vector<PredUnit> pu(mine.size());
+      for (size_t m = 0; m < mine.size(); m++) {
+        const PredCallUnit& cu = units[mine[m]];
+        const std::string unit = "unit " + std::to_string(mine[m]) + ": ";
+        const size_t n = size_t(cu.n);
+        if (cu.handle) {
+          st[m] = cu.handle->st;
+        } else {
+          st[m].preds = ex.alloc<pccb200_predictor>(n);
+          st[m].idx = ex.alloc<uint32_t>(n);
+          st[m].qw = nullptr;
+          const int32_t* dXyz = dev ? cu.xyz : to_device(ex, cu.xyz, n * 3);
+          int rc = lod_state_build(ex, *cu.lod, dXyz, cu.n, st[m], false);
+          if (rc != PCCB200_OK)
+            return fail(rc, unit + "invalid LoD parameters");
+        }
+        pu[m] = cu.pu;
+        pu[m].st = &st[m];
+        pu[m].qpo = dev || !cu.qpo ? cu.qpo : to_device(ex, cu.qpo, n * 2);
+        for (int s = 0; s < pu[m].numSets && !dev; s++) {
+          const size_t len = n * pu[m].sets[s].A;
+          pu[m].sets[s].values = to_device(ex, cu.pu.sets[s].values, len);
+          pu[m].sets[s].attrsOut = ex.alloc<int32_t>(len);
+        }
+      }
+      int bad = 0;
+      const char* why = "invalid predicting-transform parameters";
+      int rc = attr_pred_decode_on_lods(ex, int(mine.size()), pu.data(), &bad, &why);
+      if (rc != PCCB200_OK)
+        return fail(rc, "unit " + std::to_string(mine[bad]) + ": " + why);
+      for (size_t m = 0; m < mine.size() && !dev; m++)
+        for (int s = 0; s < pu[m].numSets; s++)
+          to_host(ex, units[mine[m]].pu.sets[s].attrsOut, pu[m].sets[s].attrsOut,
+                  size_t(units[mine[m]].n) * pu[m].sets[s].A);
+      return PCCB200_OK;
+    });
+  });
+}
+
+int
+check_pred_set(const pccb200_qpset* qs, const pccb200_pred_params* pp, int A, int bitdepth)
+{
+  if (!qs || !pp || (A != 1 && A != 3) || bitdepth < 1 || bitdepth > 16)
+    return PCCB200_ERR_INVALID_ARG;
+  if (qs->num_layers < 1 || qs->num_layers > PCCB200_MAX_QP_LAYERS)
+    return PCCB200_ERR_INVALID_ARG;
+  if (pp->max_num_direct_predictors < 0 || pp->max_num_direct_predictors > 3
+      || pp->adaptive_prediction_threshold < 0 || pp->adaptive_prediction_threshold > 255)
+    return PCCB200_ERR_INVALID_ARG;
+  return PCCB200_OK;
+}
+
+int
+attr_pred_multi(bool dev, int numUnits, const pccb200_lod_params* const* lods,
+                const int32_t* qnw, int numSets, const pccb200_qpset* const* qpsets,
+                const pccb200_pred_params* pred, const int32_t* A, const int32_t* bitdepth,
+                const int32_t* const* xyz, const int32_t* n, const int32_t* const* qpo,
+                const int32_t* const* values, const int8_t* const* icp, int32_t* const* out)
+{
+  if (!lods || !qnw || !qpsets || !pred || !A || !bitdepth || !xyz || !n || !values || !out
+      || numUnits <= 0 || numSets < 1 || numSets > kPredMaxSets)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer or bad size");
+  for (int s = 0; s < numSets; s++)
+    if (check_pred_set(qpsets[s], &pred[s], A[s], bitdepth[s]) != PCCB200_OK)
+      return fail(PCCB200_ERR_INVALID_ARG,
+                  "set " + std::to_string(s)
+                    + ": null pointer, bad component count, bit depth, qp layers or "
+                      "predicting-transform parameters");
+  std::vector<PredCallUnit> units(numUnits);
+  for (int u = 0; u < numUnits; u++) {
+    const std::string unit = "unit " + std::to_string(u) + ": ";
+    PredCallUnit& cu = units[u];
+    cu.n = n[u];
+    cu.xyz = xyz[u];
+    cu.qpo = qpo ? qpo[u] : nullptr;
+    cu.lod = lods[u];
+    if (!cu.lod || !cu.xyz)
+      return fail(PCCB200_ERR_INVALID_ARG, unit + "null pointer");
+    if (cu.n <= 0)
+      return fail(PCCB200_ERR_INVALID_ARG, unit + "no points");
+    for (int k = 0; k < 3; k++)
+      cu.pu.quantNeighWeight[k] = qnw[3 * u + k];
+    cu.pu.numSets = numSets;
+    for (int s = 0; s < numSets; s++) {
+      const size_t at = size_t(u) * numSets + s;
+      if (!values[at] || !out[at])
+        return fail(PCCB200_ERR_INVALID_ARG, unit + "null pointer");
+      cu.pu.sets[s] = PredSet{A[s], bitdepth[s], qpsets[s], pred[s], values[at],
+                              icp ? icp[at] : nullptr, out[at]};
+    }
+  }
+  return code_pred(dev, units);
 }
 
 }  // namespace
@@ -2292,6 +2417,59 @@ pccb200_recolour_exact_multi_batch_dev(const pccb200_recolour_params* params, in
   return recolour_multi(true, params, num_sets, num_units, d_source_xyz, n_source, d_source_attrs,
                         num_attrs, bitdepths, source_to_target_scale, tgt_to_src_offsets,
                         d_target_xyz, n_target, d_target_attrs_out, kRecolourRefExact);
+}
+
+//----------------------------------------------------------------------------
+// predicting-transform decoder (pred_pipeline.cuh)
+
+int
+pccb200_attr_pred_decode_lod(pccb200_lod_handle handle, const pccb200_qpset* qpset,
+                             const pccb200_pred_params* pred, const int32_t quant_neigh_weight[3],
+                             const int32_t* point_qp_offsets, const int8_t* icp_coeffs,
+                             const int32_t* values_in, int32_t num_attrs, int32_t bitdepth,
+                             int32_t* attrs_out)
+{
+  if (!handle || !quant_neigh_weight || !values_in || !attrs_out
+      || check_pred_set(qpset, pred, num_attrs, bitdepth) != PCCB200_OK)
+    return fail(PCCB200_ERR_INVALID_ARG, "null pointer, bad size or bad parameters");
+  if (handle->scalable)
+    return fail(PCCB200_ERR_UNSUPPORTED, "scalable lifting levels of detail");
+  std::vector<PredCallUnit> units(1);
+  PredCallUnit& cu = units[0];
+  cu.n = handle->st.n;
+  cu.qpo = point_qp_offsets;
+  cu.handle = handle;
+  for (int k = 0; k < 3; k++)
+    cu.pu.quantNeighWeight[k] = quant_neigh_weight[k];
+  cu.pu.numSets = 1;
+  cu.pu.sets[0] = PredSet{num_attrs, bitdepth, qpset, *pred, values_in, icp_coeffs, attrs_out};
+  return code_pred(false, units);
+}
+
+int
+pccb200_attr_pred_decode_multi_batch(
+  int32_t num_units, const pccb200_lod_params* const* lods, const int32_t* quant_neigh_weight,
+  int32_t num_sets, const pccb200_qpset* const* qpsets, const pccb200_pred_params* pred,
+  const int32_t* num_attrs, const int32_t* bitdepths, const int32_t* const* xyz, const int32_t* n,
+  const int32_t* const* point_qp_offsets, const int32_t* const* values_in,
+  const int8_t* const* icp_coeffs, int32_t* const* attrs_out)
+{
+  return attr_pred_multi(false, num_units, lods, quant_neigh_weight, num_sets, qpsets, pred,
+                         num_attrs, bitdepths, xyz, n, point_qp_offsets, values_in, icp_coeffs,
+                         attrs_out);
+}
+
+int
+pccb200_attr_pred_decode_multi_batch_dev(
+  int32_t num_units, const pccb200_lod_params* const* lods, const int32_t* quant_neigh_weight,
+  int32_t num_sets, const pccb200_qpset* const* qpsets, const pccb200_pred_params* pred,
+  const int32_t* num_attrs, const int32_t* bitdepths, const int32_t* const* d_xyz,
+  const int32_t* n, const int32_t* const* d_point_qp_offsets, const int32_t* const* d_values_in,
+  const int8_t* const* icp_coeffs, int32_t* const* d_attrs_out)
+{
+  return attr_pred_multi(true, num_units, lods, quant_neigh_weight, num_sets, qpsets, pred,
+                         num_attrs, bitdepths, d_xyz, n, d_point_qp_offsets, d_values_in,
+                         icp_coeffs, d_attrs_out);
 }
 
 }  // extern "C"

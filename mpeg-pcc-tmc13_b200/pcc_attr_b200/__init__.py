@@ -103,6 +103,8 @@ EXPORTS = [
     "pccb200_attr_lift_encode_multi_batch_dev", "pccb200_attr_lift_encode_multi_dev",
     "pccb200_attr_lift_encode_scalable", "pccb200_attr_lift_encode_scalable_dev",
     "pccb200_attr_lift_encode_slices", "pccb200_attr_lift_encode_slices_dev",
+    "pccb200_attr_pred_decode_lod", "pccb200_attr_pred_decode_multi_batch",
+    "pccb200_attr_pred_decode_multi_batch_dev",
     "pccb200_attr_raht_decode",
     "pccb200_attr_raht_decode_multi", "pccb200_attr_raht_decode_multi_batch",
     "pccb200_attr_raht_decode_multi_batch_dev", "pccb200_attr_raht_decode_multi_dev",
@@ -684,6 +686,93 @@ def attr_lift_decode_lod(handle, qpset, values, lcp=None, bitdepth=8, qpoffs=Non
         _p(qpoffs, C.c_int32), _p(attrs, C.c_int32), C.c_int32(a), C.c_int32(bitdepth),
         _p(values, C.c_int32), _p(l2, C.c_int8)))
     return attrs
+
+
+class PredParams(C.Structure):
+    """pccb200_pred_params: the predicting transform's APS fields of one set"""
+    _fields_ = [("max_num_direct_predictors", C.c_int32),
+                ("direct_avg_predictor_disabled", C.c_int32),
+                ("adaptive_prediction_threshold", C.c_int32),
+                ("icp_enabled", C.c_int32)]
+
+
+def _icp_row(icp):
+    """None, or a host int8 row of MAX_LODS x 3 ICP coefficients"""
+    if icp is None:
+        return None
+    row = np.zeros((MAX_LODS, 3), dtype=np.int8)
+    icp = np.asarray(icp, dtype=np.int8).reshape(-1, 3)
+    row[:len(icp)] = icp
+    return row
+
+
+def attr_pred_decode_lod(handle, qpset, pred, quant_neigh_weight, values, bitdepth=8,
+                         qpoffs=None, icp=None):
+    """pccb200_attr_pred_decode_lod: values [N, A] in coding order (as the
+    reference's loop decodes them), icp [lods, 3] or None -> decoded
+    attributes [N, A] in point order"""
+    values = np.ascontiguousarray(values, dtype=np.int32)
+    n, a = values.shape
+    out = np.zeros((n, a), dtype=np.int32)
+    if qpoffs is not None:
+        qpoffs = np.ascontiguousarray(qpoffs, dtype=np.int32)
+    qnw = (C.c_int32 * 3)(*[int(w) for w in quant_neigh_weight])
+    row = _icp_row(icp)
+    _check(lib().pccb200_attr_pred_decode_lod(
+        C.c_void_p(handle), C.byref(qpset), C.byref(pred), qnw, _p(qpoffs, C.c_int32),
+        _p(row, C.c_int8), _p(values, C.c_int32), C.c_int32(a), C.c_int32(bitdepth),
+        _p(out, C.c_int32)))
+    return out
+
+
+def _pred_multi_args(lods, qnws, qpsets, preds, comps, bitdepths, xyzs, ns, qpos, values, icps,
+                     outs):
+    m, k = len(lods), len(qpsets)
+    VP = C.c_void_p * (m * k)
+    rows = [_icp_row(r) for u in icps for r in u] if icps is not None else None
+    args = (C.c_int32(m), (C.POINTER(LodParams) * m)(*[C.pointer(lp) for lp in lods]),
+            (C.c_int32 * (3 * m))(*[int(w) for q in qnws for w in q]), C.c_int32(k),
+            (C.POINTER(QpSet) * k)(*[C.pointer(q) for q in qpsets]), (PredParams * k)(*preds),
+            (C.c_int32 * k)(*comps), (C.c_int32 * k)(*(bitdepths or [8] * k)),
+            (C.c_void_p * m)(*xyzs), (C.c_int32 * m)(*ns),
+            (C.c_void_p * m)(*qpos) if qpos is not None else None, VP(*values),
+            VP(*[None if r is None else r.ctypes.data for r in rows]) if rows is not None else None,
+            VP(*outs))
+    return args, rows
+
+
+def attr_pred_decode_multi_batch(lods, quant_neigh_weights, qpsets, preds, xyzs, values,
+                                 bitdepths=None, qpoffs=None, icps=None):
+    """pccb200_attr_pred_decode_multi_batch: lods[u], quant_neigh_weights[u]
+    (3 ints), xyzs[u] [N_u, 3], qpoffs[u] [N_u, 2] or None per unit; qpsets,
+    preds (PredParams), bitdepths per set; values[u][s] [N_u, A_s] coding order,
+    icps[u][s] [lods, 3] or None -> decoded attributes[u][s] in point order"""
+    xyzs = [np.ascontiguousarray(x, dtype=np.int32) for x in xyzs]
+    values = [[np.ascontiguousarray(v, dtype=np.int32).reshape(x.shape[0], -1) for v in u]
+              for x, u in zip(xyzs, values)]
+    outs = [[np.zeros_like(v) for v in u] for u in values]
+    qpo = None
+    if qpoffs is not None:
+        qpo = [None if q is None else np.ascontiguousarray(q, dtype=np.int32) for q in qpoffs]
+    args, _keep = _pred_multi_args(
+        lods, quant_neigh_weights, qpsets, preds, [v.shape[1] for v in values[0]], bitdepths,
+        [x.ctypes.data for x in xyzs], [x.shape[0] for x in xyzs],
+        None if qpo is None else [None if q is None else q.ctypes.data for q in qpo],
+        [v.ctypes.data for u in values for v in u], icps, [o.ctypes.data for u in outs for o in u])
+    _check(lib().pccb200_attr_pred_decode_multi_batch(*args))
+    return outs
+
+
+def attr_pred_decode_multi_batch_dev(lods, quant_neigh_weights, qpsets, preds, comps, d_xyzs, ns,
+                                     d_values, d_outs, bitdepths=None, d_qpoffs=None, icps=None):
+    """pccb200_attr_pred_decode_multi_batch_dev: device pointers (ints) d_xyzs[u],
+    d_qpoffs[u] (or None), d_values[u][s], d_outs[u][s]; comps[s] components
+    per set, ns[u] points per unit; everything else as attr_pred_decode_multi_batch"""
+    args, _keep = _pred_multi_args(
+        lods, quant_neigh_weights, qpsets, preds, comps, bitdepths, list(d_xyzs), list(ns),
+        list(d_qpoffs) if d_qpoffs is not None else None, [v for u in d_values for v in u],
+        icps, [o for u in d_outs for o in u])
+    _check(lib().pccb200_attr_pred_decode_multi_batch_dev(*args))
 
 
 def attr_lift_encode(lod_params, qpset, xyz, attrs, lcp_enabled=0, bitdepth=8, qpoffs=None):
